@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Benchmark of the weighted-MEC / PedMEC column sweep (the hot path of `whatshap phase`).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--workload cfg3] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--workload cfg3] [--impl ours|reference] [--dump-outputs DIR]
 
 One "step" = one complete forward sweep of the DP over the synthetic workload (all variant
 columns of all DP-independent blocks).  Metric: variant-columns per second (BASELINE.json).
@@ -13,6 +13,8 @@ columns of all DP-independent blocks).  Metric: variant-columns per second (BASE
              copies and super-read construction are all inside the timed region
   roofline   algorithmic bytes (SURVEY.md §8(d)) / device time of the dominant kernel vs the measured
              HBM copy bandwidth of this pool (MEASURED_PEAKS.json)
+  --dump-outputs DIR  writes the solution of the last timed step as DIR/<field>.npy (float64), for comparing two builds
+             output for output (the workload is generated from fixed seeds, so the same flags give the same inputs)
   cpu_baseline  the UNMODIFIED reference C++ (oracle/_ref) or the C restatement, single thread,
              on a bounded prefix of the same workload
 
@@ -56,11 +58,13 @@ def parse_args():
     ap.add_argument("--cols", type=int, default=None, help="override the number of variant columns")
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed as DIR/<name>.npy (float64, at most 64 MB in all)")
     return ap.parse_args()
 
 
 class ClockSampler:
-    """SM clock / throttle-reason samples DURING the timed region (B200_PROFILING.md).  The timed region of the default run is a few
+    """SM clock / throttle-reason samples DURING the timed region.  The timed region of the default run is a few
     tens of milliseconds, shorter than the start-up of an `nvidia-smi -lms` loop, so the samples are taken through NVML (the library
     nvidia-smi itself reads) every 2 ms by a thread of this process; `nvidia-smi` is the fallback when NVML cannot be loaded."""
 
@@ -162,35 +166,28 @@ def hbm_peak():
     path = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(path):
         return float(json.load(open(path))["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3), not measured"
 
 
-def recorded_traffic(workload, launches=1):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of the dominant kernel, from the committed `ncu --set full`
-    capture of this workload (profiles/traffic.json), else None.  A report that holds every big launch of one sweep (the two
-    passes of the fused pedigree sweep) is averaged over the launches of a sweep, like `algorithmic_bytes_per_launch`."""
-    path = os.path.join(ROOT, "profiles", "traffic.json")
-    if os.path.exists(path):
-        rec = json.load(open(path)).get(workload)
-        if rec:
-            per_sweep = rec.get("launches_in_report", 1) > 1
-            return rec["bytes_per_launch"] / (launches if per_sweep else 1), rec["report"]
-    return None, None
+DUMP_BUDGET = 64 * 10**6  # bytes of .npy data --dump-outputs may write
 
 
-def recorded_issue(workload, cells_per_launch, launches=1):
-    """Instruction-issue view of the same ncu capture: the DP kernels are bound by integer issue, not by HBM."""
-    path = os.path.join(ROOT, "profiles", "traffic.json")
-    if os.path.exists(path):
-        rec = json.load(open(path)).get(workload)
-        if rec and "warp_inst_executed" in rec:
-            # a report that holds every big launch of one sweep (the two passes of the fused pedigree sweep) gives totals per sweep
-            per_sweep = rec.get("launches_in_report", 1) > 1
-            inst = rec["warp_inst_executed"] / (launches if per_sweep else 1)
-            return {"issue_active_pct_of_peak": rec["issue_active_pct"], "warp_instructions_per_launch": inst,
-                    "thread_instructions_per_dp_cell": 32.0 * inst / max(cells_per_launch, 1.0),
-                    "source": rec["report"], "note": "ncu capture of one launch of the dominant kernel; 100 % = one warp instruction per scheduler per cycle"}
-    return None
+def dump_outputs(out_dir, sol):
+    """The FlatSolution the timed path returned (plan.finish() of the last step) as float64 arrays: every uint32 is exact.
+    An array larger than its share of DUMP_BUDGET is replaced by a fixed, seeded sample of its flattened elements."""
+    import numpy as np
+
+    arrays = {"cost": np.array([sol.cost])}
+    for f in ("path_index", "path_tv", "partition", "sr_allele", "sr_quality"):
+        arrays[f] = np.asarray(getattr(sol, f))
+    share = DUMP_BUDGET // len(arrays)
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        a = a.astype(np.float64)
+        if a.nbytes > share:
+            keep = np.sort(np.random.default_rng(0).choice(a.size, share // a.itemsize, replace=False))
+            a = a.reshape(-1)[keep]
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 def make_workload(name, cols, rank):
@@ -322,6 +319,8 @@ def main():
     world = int(os.environ.get("WORLD_SIZE", "1"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
     if args.impl == "reference":
+        if args.dump_outputs:
+            raise SystemExit("--dump-outputs writes what the CUDA path computed; --impl reference times the CPU reference only")
         bench_reference(args, rank, world)
         return
 
@@ -339,7 +338,7 @@ def main():
     name = args.workload
     prob = make_workload(name, args.cols, rank)
     n_cols = prob.n_cols
-    flush = torch.empty(512 << 20, dtype=torch.uint8, device="cuda")  # > 126 MB L2
+    flush = torch.empty(512 << 20, dtype=torch.uint8, device="cuda")  # 10x the 50 MB L2 of an H100
 
     def barrier():
         torch.cuda.synchronize()
@@ -385,7 +384,7 @@ def main():
     _lib.solve(prob, device=local_rank)  # warm-up (context, allocator)
     barrier()
     e2e_t0 = time.perf_counter()
-    e2e_steps = max(1, min(args.steps, 3))
+    e2e_steps = max(1, args.steps)
     for _ in range(e2e_steps):
         sol2, st2 = _lib.solve(prob, device=local_rank)
     barrier()
@@ -448,18 +447,6 @@ def main():
         peak, peak_src = hbm_peak()
         launches = int(stats["kernel_launches"])
         achieved = stats["algorithmic_bytes"] / (statistics.mean(sweep_ms) / 1e3) / 1e9
-        issue = recorded_issue(name, stats["cells"] / max(launches, 1), launches)
-        roofline_issue = None
-        if issue and clocks.get("sm_mhz"):
-            # warp instructions of one sweep (ncu capture of one launch x launches) against what the SMs can issue in that time
-            sms = torch.cuda.get_device_properties(local_rank).multi_processor_count
-            peak_issue = sms * 4 * clocks["sm_mhz"] * 1e6  # one warp instruction per scheduler and cycle
-            ach = issue["warp_instructions_per_launch"] * launches / (statistics.mean(sweep_ms) / 1e3)
-            roofline_issue = {"bound": "int-issue", "achieved": ach, "peak": peak_issue, "unit": "warp-instructions/s", "frac": ach / peak_issue,
-                              "thread_instructions_per_dp_cell": issue["thread_instructions_per_dp_cell"], "source": issue["source"],
-                              "note": "the bound that binds: the DP kernels issue integer min / add instructions, one warp instruction per "
-                                      "scheduler and cycle at best; instruction count from the committed ncu capture of this kernel, time "
-                                      "from this run"}
         line = {
             "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": args.steps, "warmup": max(args.warmup, 3),
             "ms_per_step": max_ms / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
@@ -474,20 +461,18 @@ def main():
             },
             "roofline": {
                 "bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                "traffic": recorded_traffic(name, launches)[0], "traffic_source": recorded_traffic(name, launches)[1], "peak_source": peak_src,
+                "peak_source": peak_src,
                 "algorithmic_bytes_per_launch": stats["algorithmic_bytes"] / max(launches, 1),
                 "kernel": {1: "tile_panel_kernel", 2: "col_direct_kernel", 3: "ped_fused_kernel" if launches == 3 else "col_batched_kernel"}.get(int(stats["path_kind"]), "col_direct_kernel"),
-                "issue": issue,
                 "algorithmic_bytes_per_step": int(stats["algorithmic_bytes"]), "launches_per_step": launches,
                 "bytes_moved_per_step": {"backpointers": int(stats["backptr_bytes"]), "state": int(stats["state_bytes"])},
                 "note": ("algorithmic bytes follow the reference's data layout (u32 projection read + u32 value and u32 back-pointer "
                          "written per entry and column, SURVEY.md 8(d)); the tile kernel keeps the projection in shared memory for a "
-                         "whole panel of columns and stores 1-bit back-pointers, so its real DRAM traffic (`traffic`, ncu) is far below "
+                         "whole panel of columns and stores 1-bit back-pointers, so its real DRAM traffic is far below "
                          "that and frac can exceed 1: the kernel is bound by integer issue, see dp_cells_per_s"),
                 "dp_cells_per_s": stats["cells"] / (statistics.mean(sweep_ms) / 1e3),
                 "sweep_ms": statistics.mean(sweep_ms), "backtrace_ms": statistics.mean(step_ms) - statistics.mean(sweep_ms),
             },
-            "roofline_issue": roofline_issue,
             "clocks": clocks,
             "e2e_api": e2e_api,
             "e2e": {"value": e2e_value, "unit": UNIT, "h2d_bytes_per_step": int(st2["h2d_bytes"]), "d2h_bytes_per_step": int(st2["d2h_bytes"]),
@@ -500,6 +485,8 @@ def main():
             line["e2e_sharded"] = sharded
         if not args.no_cpu_baseline and world == 1:
             line["cpu_baseline"] = run_cpu_baseline(name, prob)
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, sol)
         print(json.dumps(line), flush=True)
     if world > 1:
         dist.destroy_process_group()

@@ -1,5 +1,5 @@
 /*
- * whmec.h — C ABI of the B200-native weighted-MEC / PedMEC dynamic program.
+ * whmec.h — C ABI of the CUDA (sm_90a) weighted-MEC / PedMEC dynamic program.
  *
  * This is the drop-in boundary for ONE hot path of WhatsHap: the PedigreeDPTable
  * column sweep.  The reference exposes that path as a C++ class bound through

@@ -1,6 +1,6 @@
 """Builds integration/whatshap_bridge.pyx against a WhatsHap source tree, out of this repository's tree.
     python integration/build_bridge.py [whatshap source dir] [output dir]
-Defaults: the scratch copy that oracle/build_pyref.py makes of /root/reference (authoring container) and its
+Defaults: the scratch copy that oracle/build_pyref.py makes of the WhatsHap tree at $WHATSHAP_REF and its
 own directory, so that `import whatshap_bridge` works wherever `import whatshap` does.  Nothing is copied from
 WhatsHap: its .pxd files and C++ headers are only on the include paths."""
 import os

@@ -1,7 +1,6 @@
-"""TEST INFRASTRUCTURE (authoring container only): builds the reference's own Python extension
-`whatshap.core` from /root/reference in a scratch directory OUTSIDE this repository so that tests can
-drive the real Cython classes.  Nothing is copied into the repo and the build does not travel to the
-GPU box (a Python reference cannot travel; its outputs are the golden vectors under tests/golden/).
+"""TEST INFRASTRUCTURE (only where a WhatsHap source tree is at $WHATSHAP_REF): builds the reference's own Python
+extension `whatshap.core` in a scratch directory OUTSIDE this repository so that tests can drive the real Cython
+classes.  Nothing is copied into the repo; where the reference is absent, its answers stored under tests/golden/ stand in.
 
 Recipe (SURVEY.md Appendix B): copy src/ whatshap/ setup.py, stub _version.py, skip the polyphase solver
 import (needs `pulp`), build_ext --inplace with the distribution compiler (/usr/bin/g++; /opt/gcc links
@@ -52,8 +51,8 @@ SHIP = os.path.join(os.path.dirname(os.path.abspath(__file__)), "_ref", "pyref")
 
 
 def ship() -> str:
-    """Puts the COMPILED reference binding where it travels to the GPU box (oracle/_ref is git-ignored, not
-    gpurun-ignored, exactly like oracle/_ref/libwhref.so): oracle/_ref/pyref/whatshap/core.*.so plus two stub modules
+    """Puts the COMPILED reference binding next to oracle/_ref/libwhref.so (oracle/_ref is git-ignored):
+    oracle/_ref/pyref/whatshap/core.*.so plus two stub modules
     of our own (`__init__`, `variant` — core.pyx imports `.variant.Variant`, a three-field dataclass).  No reference
     source is copied.  Returns the directory to put on sys.path ('' when neither a build nor a prebuilt copy exists)."""
     pkg = os.path.join(SHIP, "whatshap")
@@ -78,7 +77,7 @@ def ship() -> str:
 
 
 def shipped_core():
-    """The compiled reference binding `whatshap.core` (authoring container or prebuilt copy on the GPU box), or None."""
+    """The compiled reference binding `whatshap.core` (built here or a prebuilt copy under oracle/_ref), or None."""
     if "whatshap.core" in sys.modules:  # already imported (e.g. from the full out-of-tree build): the same binding
         return sys.modules["whatshap.core"]
     path = ship()

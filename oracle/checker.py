@@ -22,8 +22,8 @@ REF_SO = os.path.join(HERE, "_ref", "libwhref.so")
 
 
 def build(quiet: bool = True) -> None:
-    """Compile the checkers (oracle/Makefile).  The reference build is skipped where
-    /root/reference is absent (GPU box): the prebuilt _ref/libwhref.so is used as is."""
+    """Compile the checkers (oracle/Makefile).  The reference build is skipped where the WhatsHap
+    sources ($WHATSHAP_REF) are absent: a prebuilt _ref/libwhref.so is used as is."""
     subprocess.run(["make", "-C", HERE], check=True, capture_output=quiet)
 
 

@@ -2,7 +2,7 @@
  * TEST INFRASTRUCTURE — NOT PART OF THE PRODUCT PATH.
  *
  * Plain-C restatement of WhatsHap's forward-backward genotyping DP (GenotypeDPTable), the checker of
- * whmec_genotype (tests/, scripts/gpu_genotype_check.py).  Nothing under whatshap_b200/ links, imports or
+ * whmec_genotype (tests/).  Nothing under whatshap_b200/ links, imports or
  * executes this file.
  *
  * Parity status: PINNED within floating-point tolerance.  Validated against the compiled, unmodified

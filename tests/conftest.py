@@ -10,7 +10,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with -m gpu)")
 
 
 @pytest.fixture(scope="session")
@@ -33,7 +33,7 @@ def gpu():
     """The CUDA library; GPU tests fail loudly (not skip) when it cannot run."""
     from whatshap_b200 import _lib
 
-    assert _lib.device_count() > 0, "no CUDA device visible: GPU tests must run on the B200 box"
+    assert _lib.device_count() > 0, "no CUDA device visible: GPU tests must run on an H100"
     return _lib
 
 

@@ -2,7 +2,7 @@
 //
 // Runs pack.cpp and the __host__ __device__ per-thread functions of dp_device.h (the same code
 // the CUDA kernels execute) serially on the CPU so that their logic can be checked against the
-// oracle in the GPU-less authoring container.  It is built into tests/emul/libwhemul.so by
+// oracle on a machine without a GPU.  It is built into tests/emul/libwhemul.so by
 // tests/emul/Makefile, loaded only by tests/test_emulation.py, and is NOT a fallback: the product
 // library (whatshap_b200/csrc) contains no CPU execution path.
 #include <algorithm>

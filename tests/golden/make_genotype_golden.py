@@ -1,6 +1,6 @@
 """Generates tests/golden/genotype.npz: flat problems and the genotype likelihoods the UNMODIFIED reference
-GenotypeDPTable (oracle/_ref/libwhref.so: whref_genotype, compiled in place from /root/reference by oracle/Makefile)
-computes for them, rounded from long double to double.  Run in the authoring container:
+GenotypeDPTable (oracle/_ref/libwhref.so: whref_genotype, compiled in place from $WHATSHAP_REF by oracle/Makefile)
+computes for them, rounded from long double to double.  Run in the machine with the reference:
     python tests/golden/make_genotype_golden.py
 
 Cases

@@ -1,6 +1,6 @@
 """Generates tests/golden/*.npz: inputs (flat problems) and the outputs of the UNMODIFIED
-reference C++ PedigreeDPTable (oracle/_ref/libwhref.so, compiled in place from /root/reference by
-oracle/Makefile) on them.  Run in the authoring container:  python tests/golden/make_golden.py
+reference C++ PedigreeDPTable (oracle/_ref/libwhref.so, compiled in place from $WHATSHAP_REF by
+oracle/Makefile) on them.  Run in the machine with the reference:  python tests/golden/make_golden.py
 
 Groups
   reference_cases   the read matrices / pedigrees of the reference's own tests

@@ -1,6 +1,6 @@
 """Generates tests/golden/readselect.npz with the UNMODIFIED reference: `whatshap.readselect.readselection`
-and `whatshap.priorityqueue.PriorityQueue`, built out of tree by oracle/build_pyref.py (authoring
-container only -- a Python reference cannot travel to the GPU box, its outputs can).
+and `whatshap.priorityqueue.PriorityQueue`, built out of tree by oracle/build_pyref.py from the
+WhatsHap tree at $WHATSHAP_REF (a Python reference cannot travel to a machine without it, its outputs can).
     python tests/golden/make_readselect_golden.py
 
 Contents

@@ -1,4 +1,6 @@
-"""Loader for the reference-generated golden vectors (tests/golden/make_golden.py)."""
+"""Loader for the reference-generated golden vectors (tests/golden/make_golden.py) and for stored answers of the
+reference's Python binding (`reference_answer`)."""
+import json
 import os
 
 import numpy as np
@@ -42,3 +44,25 @@ def check(solve, group):
             assert got.same_as(want), (label, got.diff(want))
         n += 1
     return n
+
+
+_ANSWERS = {}
+
+
+def reference_answer(module, key, live=None):
+    """The reference's answer `key`, stored in tests/golden/<module>_answers.json.  Where the reference binding is
+    available the caller passes its `live` answer (JSON-like): it must equal the stored copy, and WHMEC_RECORD_GOLDEN=1
+    stores it instead.  Elsewhere the stored copy stands for the reference."""
+    path = os.path.join(HERE, module + "_answers.json")
+    if path not in _ANSWERS:
+        _ANSWERS[path] = json.load(open(path)) if os.path.exists(path) else {}
+    stored = _ANSWERS[path]
+    if live is not None:
+        live = json.loads(json.dumps(live))
+        if os.environ.get("WHMEC_RECORD_GOLDEN") == "1":
+            stored[key] = live
+            with open(path, "w") as f:
+                json.dump(stored, f, sort_keys=True, separators=(",", ":"))
+        assert stored.get(key) == live, f"{key}: the reference's answer differs from the stored one in {path}"
+    assert key in stored, f"{key}: no stored answer of the reference in {path}"
+    return stored[key]

@@ -1,7 +1,7 @@
 """pytest plugin used by test_reference_suite_with_swapin.py (second run): the reference's test modules import
 `whatshap.core`; before they do, EVERY class of this path in that module is replaced by this repository's Python
 mirror (`whatshap_b200.core`), `whatshap.graph.ComponentFinder` by `whatshap_b200.components.ComponentFinder`, and the
-CUDA solves behind `PedigreeDPTable` / `GenotypeDPTable` by the CPU checker (no GPU in the authoring container; the CUDA solve is held to the
+CUDA solves behind `PedigreeDPTable` / `GenotypeDPTable` by the CPU checker (no GPU in the machine with the reference; the CUDA solve is held to the
 same checker by the GPU tests).  The reference's tests then exercise this package's containers unmodified."""
 import os
 import sys

@@ -28,7 +28,7 @@ def test_library_exports_every_declared_symbol():
     for name in declared_symbols():
         assert hasattr(lib, name), name
     assert lib.whmec_abi_version() == 2
-    assert b"sm_100a" in lib.whmec_build_info()
+    assert b"sm_90a" in lib.whmec_build_info()
 
 
 def test_struct_layout_matches_header(tmp_path):

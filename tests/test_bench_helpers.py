@@ -1,7 +1,6 @@
-"""bench.py pieces that run without a GPU: the clock sampler degrades to an explicit "no sampler" record instead of failing, the
-issue / traffic records of profiles/traffic.json are read per launch (a multi-launch sweep is averaged over its launches)."""
+"""bench.py pieces that run without a GPU: the clock sampler degrades to an explicit "no sampler" record instead of failing,
+--dump-outputs writes the solution as float64 arrays within its size budget."""
 import importlib.util
-import json
 import os
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -24,16 +23,25 @@ def test_clock_sampler_without_nvml_or_nvidia_smi():
     assert rec["samples"] == 0 or rec["sm_mhz"] is not None  # either nothing could be sampled (this box) or real samples
 
 
-def test_traffic_records_are_per_launch():
+def test_dump_outputs_writes_the_solution_as_float64(tmp_path):
+    import numpy as np
+
+    from whatshap_b200._abi import FlatSolution
+
     bench = load_bench()
-    rec = json.load(open(os.path.join(ROOT, "profiles", "traffic.json")))
-    for name in ("cfg2", "cfg3", "cfg4", "cfg5"):
-        assert name in rec and rec[name]["warp_inst_executed"] > 0 and rec[name]["report"].endswith(".ncu-rep")
-    # cfg5's report holds both passes of the fused pedigree sweep: totals of the sweep, divided by the launches of a sweep
-    assert rec["cfg5"]["launches_in_report"] == 2
-    per_launch, report = bench.recorded_traffic("cfg5", 3)
-    assert abs(per_launch * 3 - rec["cfg5"]["bytes_per_launch"]) < 1 and report == rec["cfg5"]["report"]
-    issue = bench.recorded_issue("cfg5", 1e9, 3)
-    assert abs(issue["warp_instructions_per_launch"] * 3 - rec["cfg5"]["warp_inst_executed"]) < 1
-    one, _ = bench.recorded_traffic("cfg3", 36)
-    assert one == rec["cfg3"]["bytes_per_launch"]
+    sol = FlatSolution(5, 3, 1)
+    sol.cost = 4294967295
+    sol.path_index[:] = [0, 1, 2, 3, 4]
+    sol.partition[:] = [1, 0, 1]
+    bench.dump_outputs(str(tmp_path), sol)
+    got = {p.stem: np.load(p) for p in tmp_path.glob("*.npy")}
+    assert set(got) == {"cost", "path_index", "path_tv", "partition", "sr_allele", "sr_quality"}
+    assert all(a.dtype == np.float64 for a in got.values())
+    assert got["cost"].tolist() == [4294967295.0] and got["path_index"].tolist() == [0, 1, 2, 3, 4]
+    assert got["sr_allele"].shape == (1, 2, 5)
+    bench.DUMP_BUDGET = 6 * 16  # two float64 values per array: larger arrays become a fixed sample of their elements
+    bench.dump_outputs(str(tmp_path), sol)
+    a, b = np.load(tmp_path / "path_index.npy"), np.load(tmp_path / "sr_allele.npy")
+    assert a.shape == (2,) and set(a.tolist()) <= {0, 1, 2, 3, 4} and b.shape == (2,)
+    bench.dump_outputs(str(tmp_path), sol)
+    assert np.array_equal(np.load(tmp_path / "path_index.npy"), a)

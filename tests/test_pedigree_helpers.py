@@ -1,6 +1,6 @@
 """Recombination costs in, recombination events out (whatshap_b200/pedigree.py): the reference's known answers
 (tests/test_pedigreephasing.py:432-441, tests/test_pedigree.py:53-80), values recorded from the unmodified
-reference module, and a live comparison with it in the authoring container."""
+reference module, and a live comparison with it in the machine with the reference."""
 import os
 import sys
 
@@ -77,7 +77,7 @@ def test_same_numbers_as_the_reference_module():
 
     path = build_pyref.build()
     if not path:
-        pytest.skip("the reference tree is not available here (GPU box): recorded values cover this")
+        pytest.skip("the reference tree is not available here: recorded values cover this")
     sys.path.insert(0, path)
     import whatshap.pedigree as ref
 

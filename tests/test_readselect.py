@@ -1,6 +1,6 @@
 """Coverage-capping read selection (SURVEY.md §8(f) rank 3): the reference's known answers
 (tests/test_readselect.py:5-108), golden vectors produced by the unmodified reference module
-(tests/golden/make_readselect_golden.py) and, where the reference can be built (authoring container),
+(tests/golden/make_readselect_golden.py) and, where the reference can be built (machine with the reference),
 a live comparison with it -- the SAME reads must be selected, ties included."""
 import os
 import sys
@@ -136,7 +136,7 @@ def test_selection_respects_the_coverage_cap():
     assert len(chosen) < len(reads) // 3
 
 
-# ---- live comparison with the reference module (authoring container only) ----
+# ---- live comparison with the reference module (only where the reference is available) ----
 @pytest.fixture(scope="module")
 def reference_modules():
     sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -144,7 +144,7 @@ def reference_modules():
 
     path = build_pyref.build()
     if not path:
-        pytest.skip("the reference tree is not available here (GPU box): golden vectors cover this")
+        pytest.skip("the reference tree is not available here: golden vectors cover this")
     sys.path.insert(0, path)
     import whatshap.core
     import whatshap.readselect

@@ -1,4 +1,4 @@
-"""whatshap_b200 — B200-native weighted-MEC / PedMEC dynamic program behind WhatsHap's
+"""whatshap_b200 — CUDA (H100, sm_90a) weighted-MEC / PedMEC dynamic program behind WhatsHap's
 `PedigreeDPTable` interface.  See DESIGN.md; the compute path is CUDA only (libwhmec.so)."""
 from .core import (  # noqa: F401
     Genotype,

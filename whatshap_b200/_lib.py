@@ -48,7 +48,7 @@ EXPORTS = (
 
 
 def build(verbose: bool = False) -> str:
-    """Compile libwhmec.so in-tree for sm_100a (nvcc cross-compiles without a GPU)."""
+    """Compile libwhmec.so in-tree for sm_90a (nvcc cross-compiles without a GPU)."""
     res = subprocess.run(["make", "-C", os.path.join(HERE, "csrc")], capture_output=not verbose, text=True)
     if res.returncode != 0:
         raise RuntimeError("building libwhmec.so failed:\n" + (res.stdout or "") + (res.stderr or ""))

@@ -36,8 +36,7 @@ constexpr uint32_t STAGE_PAD_WORDS = BULK_SKEW << BULK_MAX_GA;
 
 // Arrivals at the split column barrier.  1 (default): every thread arrives -- its release covers its own stores, which is also
 // what compute-sanitizer's racecheck can follow (0 hazards); 0: one arrival per warp (lane 0 after __syncwarp: correct by
-// cumulativity, but racecheck then reports the other lanes' stores as unordered; measured 0.4 % faster: 8.85 vs 8.88 ms per
-// cfg3 sweep, profiles/r02/r02n_*).
+// cumulativity, but racecheck then reports the other lanes' stores as unordered).
 #ifndef WHMEC_COL_ARRIVE_ALL
 #define WHMEC_COL_ARRIVE_ALL 1
 #endif
@@ -64,7 +63,7 @@ struct TileSmem {
     uint32_t a_col[TC_CHUNK];
     uint32_t panel_index;
 };
-static_assert(sizeof(TileSmem) <= 227 * 1024, "TileSmem exceeds the shared memory of one CTA on sm_100");
+static_assert(sizeof(TileSmem) <= 227 * 1024, "TileSmem exceeds the shared memory of one CTA on sm_90");
 
 // The steady-state column of a coverage-capped ReadSet: the oldest local read (local bit 0) ends and
 // there are enough outputs for every thread.  The planner marks such columns (TileCol::pad0):
@@ -737,7 +736,7 @@ struct TileImpl {
     uint32_t *d_state = nullptr, *d_arena = nullptr, *d_chain_begin = nullptr;
     unsigned long long *d_chain_keys = nullptr;
     uint32_t n_chains = 0;
-    uint32_t n_sm = 148;
+    uint32_t n_sm = 132;
 };
 
 }  // namespace
@@ -905,7 +904,7 @@ int TilePlan::create(const Packed &pk, cudaStream_t stream, uint64_t &h2d, std::
     // exhausted) the same calls go through the driver's bounce buffer
     for (const Piece &q : pieces) CUDA_TRY(up(q.dst, q.src, q.bytes));
     {
-        int dev = 0, sms = 148;
+        int dev = 0, sms = 132;
         CUDA_TRY(cudaGetDevice(&dev));
         CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
         I->n_sm = (uint32_t)sms;

@@ -29,7 +29,7 @@ void plan_tiles(const Packed &pk, TileSchedule &ts) {
     }
     const bool timing = std::getenv("WHMEC_TIMING") != nullptr;
     const char *packed_env = std::getenv("WHMEC_TILE_PACKED_BP");
-    const bool packed_bp = !(packed_env && packed_env[0] == '0');  // default since round 2 (B200: 29.97 -> 25.42 ms on cfg3); "0" keeps the warp-ballot layout
+    const bool packed_bp = !(packed_env && packed_env[0] == '0');  // the default; "0" keeps the warp-ballot layout
     const char *mirror_env = std::getenv("WHMEC_TILE_MIRROR");
     const bool mirror_on = !(mirror_env && mirror_env[0] == '0');  // "0": every tile of every panel is computed (test hook)
     auto tnow = [] { return std::chrono::steady_clock::now(); };

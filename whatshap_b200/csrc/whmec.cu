@@ -1,4 +1,4 @@
-// C ABI (include/whmec.h) + CUDA kernels of the weighted-MEC / PedMEC column sweep for sm_100a.
+// C ABI (include/whmec.h) + CUDA kernels of the weighted-MEC / PedMEC column sweep for sm_90a.
 //
 // Replaces, behind plain C entry points, the work of PedigreeDPTable's constructor
 // (src/pedigreedptable.cpp:15-37 -> compute_table :84-174 -> compute_column :177-335) and of
@@ -512,7 +512,7 @@ __global__ void __launch_bounds__(PF_THREADS, 1) ped_fused_kernel(const PedFused
     if (tid < PF_T) a.out_vecs[(size_t)c * PF_T + tid] = R[tid] < PF_INF ? R[tid] : UMAX;  // a chain ends with f == 0
 }
 
-// ---- the same sweep with a CLUSTER of CTAs per chain (fewer chains than SMs: cfg5 has 40 chains for 148 SMs, a table segment
+// ---- the same sweep with a CLUSTER of CTAs per chain (fewer chains than SMs: cfg5 has 40 chains for 132 SMs, a table segment
 // on one of 8 GPUs five).  Every CTA of the cluster holds the whole previous column (transition minima M + argmins A, double
 // buffered) and the column's tables; a large column's outputs are split between the CTAs, and the thread that finishes an
 // output forms its transition minima from registers and writes that row into the NEXT-column buffer of every CTA of the
@@ -930,8 +930,7 @@ struct DevBuf {
 // ---- page-locked staging blocks: the memory behind StagedVec (hostpool.h) ------------------------------------------------
 // The packer and the planner write the arrays that are uploaded as they are (per-column records, cost functions, panels)
 // straight into page-locked blocks, so that an upload is one asynchronous DMA transfer per array: from pageable memory
-// cudaMemcpyAsync goes through the driver's bounce buffer and blocks the calling thread (B200 box: 2.5 ms for the 18.8 MB
-// of cfg3, up to 8 ms for the cost functions of cfg5).  Blocks are kept for the life of the process and reused
+// cudaMemcpyAsync goes through the driver's bounce buffer and blocks the calling thread for the whole copy.  Blocks are kept for the life of the process and reused
 // (cudaHostAlloc costs milliseconds); small arrays stay on the heap.  WHMEC_PINNED_UPLOAD=0 switches the pool off (test hook).
 struct PinnedPool {
     struct Block {
@@ -1299,7 +1298,7 @@ int plan_create_impl(const whmec_problem *p, int device, whmec_plan *pl, std::st
             CUDA_TRY(cudaFuncSetAttribute(ped_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PF_SMEM));
             CUDA_TRY(cudaFuncSetAttribute(ped_fused_cluster_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PF_CLUSTER_SMEM));
             {   // fewer chains than SMs: a cluster of 2 / 4 / 8 CTAs per chain (WHMEC_PED_CLUSTER=n forces n, 1 = off)
-                int dev = 0, sms = 148;
+                int dev = 0, sms = 132;
                 CUDA_TRY(cudaGetDevice(&dev));
                 CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
                 uint32_t cs = 1;
@@ -1874,7 +1873,7 @@ extern "C" {
 
 int whmec_abi_version(void) { return WHMEC_ABI_VERSION; }
 
-const char *whmec_build_info(void) { return "whmec: CUDA sm_100a weighted-MEC/PedMEC DP (column + tile kernels), no CPU path"; }
+const char *whmec_build_info(void) { return "whmec: CUDA sm_90a weighted-MEC/PedMEC DP (column + tile kernels), no CPU path"; }
 
 int whmec_device_count(void) {
     int n = 0;
