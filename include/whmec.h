@@ -41,7 +41,7 @@ extern "C" {
 #define WHMEC_ERR_MENDELIAN 1   /* "Error: Mendelian conflict"   (pedigreedptable.cpp:301-303) */
 #define WHMEC_ERR_INPUT 2       /* unsorted reads / malformed arrays (columniterator.cpp:29,32) */
 #define WHMEC_ERR_CUDA 3        /* CUDA runtime failure, message in err */
-#define WHMEC_ERR_UNSUPPORTED 4 /* > 32 active reads (graycodes.cpp:12), cost range, HBM budget */
+#define WHMEC_ERR_UNSUPPORTED 4 /* > 32 active reads (graycodes.cpp:12), cost range, a column beyond the HBM budget */
 
 /* allele codes in ent_allele (src/entry.h:8) */
 #define WHMEC_ALLELE_REF 0

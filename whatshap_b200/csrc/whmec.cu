@@ -24,6 +24,7 @@
 #include <vector>
 
 #include "../../include/whmec.h"
+#include "bounded.h"
 #include "common.h"
 #include "dp_device.h"
 #include "ped_fused.h"
@@ -394,6 +395,7 @@ struct PedFusedArgs {
     const uint32_t *in_vecs;  // [chains][4] true inputs (pass 2)
     uint32_t *out_vecs;       // [chains][4]: pass 1: row 0 of the chain's transfer matrix; pass 2: the chain's true output
     uint32_t unit;            // 1: pass 1 (input e_0, values only), 0: pass 2
+    uint32_t chain0;          // block (cluster) b sweeps chain chain0 + b: a segment of the memory-bounded sweep
 };
 
 constexpr uint32_t PF_MAX_ENT = PF_T << PF_MAX_F;
@@ -441,7 +443,7 @@ __global__ void __launch_bounds__(PF_THREADS, 1) ped_fused_kernel(const PedFused
     uint32_t *R = M + PF_MAX_ENT;                                       // raw values of the current column [2^f][4]
     uint8_t *A = reinterpret_cast<uint8_t *>(R + PF_MAX_ENT);           // argmins belonging to M
     unsigned long long *keys = reinterpret_cast<unsigned long long *>(R + PF_MAX_ENT / 2);  // small columns only (< 4096 entries)
-    const uint32_t tid = threadIdx.x, c = blockIdx.x;
+    const uint32_t tid = threadIdx.x, c = a.chain0 + blockIdx.x;
     const uint32_t k0 = a.chain_begin[c], k1 = a.chain_begin[c + 1];
     const bool write_bp = !a.unit;
     pf_stage_column(C, a, c, k0, k0, k1, M, A, tid);
@@ -529,7 +531,7 @@ __global__ void __launch_bounds__(PF_THREADS, 1) ped_fused_cluster_kernel(const 
     PedFusedCol &C = *reinterpret_cast<PedFusedCol *>(pf_raw);
     uint32_t *Mb = reinterpret_cast<uint32_t *>(pf_raw + PF_COL_BYTES);     // [2][PF_MAX_ENT]
     uint8_t *Ab = reinterpret_cast<uint8_t *>(Mb + 2 * PF_MAX_ENT);          // [2][PF_MAX_ENT]
-    const uint32_t tid = threadIdx.x, c = blockIdx.x / cs;
+    const uint32_t tid = threadIdx.x, c = a.chain0 + blockIdx.x / cs;
     const uint32_t k0 = a.chain_begin[c], k1 = a.chain_begin[c + 1];
     const bool write_bp = !a.unit;
     pf_stage_column(C, a, c, k0, k0, k1, Mb, Ab, tid);
@@ -878,8 +880,10 @@ __global__ void __launch_bounds__(32) bt_exits_kernel(const BtArgs a, uint32_t *
     if (threadIdx.x == 0) exits[idx] = out;
 }
 
+// carry (memory-bounded sweep, chains of one segment): in: the value handed over by the segment to the right (entry >= 0);
+// out: the value this segment hands to the one on its left
 __global__ void bt_entries_kernel(const BtArgs a, const uint32_t *__restrict__ exits, uint32_t *__restrict__ entries,
-                                  uint32_t *__restrict__ seg_exits) {
+                                  uint32_t *__restrict__ seg_exits, uint32_t *__restrict__ carry = nullptr) {
     const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
     if (seg_exits) {
         if (t >= a.T) return;
@@ -889,11 +893,12 @@ __global__ void bt_entries_kernel(const BtArgs a, const uint32_t *__restrict__ e
         return;
     }
     if (t) return;
-    uint32_t e = a.entry < 0 ? 0u : (uint32_t)a.entry;  // the optimum's exit is stored for every u alike
+    uint32_t e = a.entry < 0 ? 0u : (carry ? *carry : (uint32_t)a.entry);  // the optimum's exit is stored for every u alike
     for (uint32_t c = a.n_chains; c-- > 0;) {
         entries[c] = e;
         e = exits[c * a.T + e];
     }
+    if (carry) *carry = e;
 }
 
 // one warp per chain
@@ -906,7 +911,43 @@ __global__ void __launch_bounds__(32) bt_paths_kernel(const BtArgs a, const uint
     uint32_t x, tv, ptv, cost = 0;
     bt_chain_start(a, bv, c, entries[c], &x, &tv, &ptv, &cost);
     backtrace_range_warp(bv, S, a.chain_begin[c + 1] - 1, a.chain_begin[c], x, tv, ptv, path_index, path_tv);
-    if (c + 1 == a.n_chains && threadIdx.x == 0) result[0] = cost;
+    if (result && c + 1 == a.n_chains && threadIdx.x == 0) result[0] = cost;
+}
+
+// Memory-bounded sequential sweep: one warp walks the columns [k_lo, k_hi] of one segment, whose back-pointers are in the arena
+// (chain boundaries inside are crossed as backtrace_range crosses them).  last_vals != nullptr: k_hi is the table's last column,
+// the walk starts at its optimum and writes the cost.  Otherwise it continues the walk of the segment to the right from the
+// state that walk left: state[0] = the cell of column k_hi + 1, state[1] = the transmission value handed to column k_hi.
+// Either way it leaves (cell of k_lo, value handed to k_lo - 1) in state for the segment to the left.
+__global__ void __launch_bounds__(32) bt_segment_kernel(const BtView v, uint32_t k_hi, uint32_t k_lo, const uint32_t *__restrict__ last_vals,
+                                                        uint32_t *__restrict__ state, uint32_t *__restrict__ path_index,
+                                                        uint32_t *__restrict__ path_tv, uint32_t *__restrict__ result) {
+    __shared__ BtWarpSmem S;
+    uint32_t x, tv, ptv;
+    if (last_vals) {
+        uint32_t cost;
+        if (v.T == 1) {  // as backtrace_kernel
+            const ColMeta &m = v.cols[k_hi];
+            x = candidate_index(m, 0, bp_load(v.arena, m.bp_off, m.bp_width, 0));
+            tv = ptv = 0;
+            cost = last_vals[0];
+        } else {  // as bt_chain_start for the table's last chain
+            pick_optimum(v.cols[k_hi], last_vals, v.arena, v.T, v.tb, &cost, &x, &tv, &ptv);
+        }
+        if (threadIdx.x == 0) result[0] = cost;
+    } else {  // the step of backtrace_range from column k_hi + 1 into k_hi
+        const uint32_t xn = state[0];
+        tv = state[1];
+        const uint32_t b = xn & low_mask(v.cols[k_hi + 1].bw);
+        const ColMeta &pm = v.cols[k_hi];
+        x = backpointer_to_index(pm, v.tb, b, bp_load(v.arena, pm.bp_off, pm.bp_width, (uint64_t)b * v.T + tv), &ptv);
+    }
+    const uint32_t out = backtrace_range_warp(v, S, k_hi, k_lo, x, tv, ptv, path_index, path_tv);
+    __syncwarp();
+    if (threadIdx.x == 0) {  // lane 0 wrote path_index[k_lo] itself
+        state[0] = path_index[k_lo];
+        state[1] = out;
+    }
 }
 
 // Device buffers come from the device's stream-ordered memory pool with an unlimited release
@@ -1134,6 +1175,15 @@ struct whmec_plan {
     DevBuf<uint32_t> d_chain_rows, d_chain_in, d_chain_out;
     uint32_t sweeps_done = 0;
     cudaGraphExec_t graph_exec = nullptr;
+    // memory-bounded sweep (back-pointers beyond the budget, DESIGN §4.3): segments share one arena (ColMeta::bp_off rebased to the
+    // segment's first column); the sweep leaves the last segment's back-pointers there, the backtrace sweeps the others right to left
+    bool bounded = false;
+    std::vector<uint32_t> seg_col;    // sequential path: column cuts, segment s = columns [seg_col[s], seg_col[s + 1])
+    std::vector<uint64_t> seg_ckpt;   // sequential path: word offset in d_ckpt of the values column seg_col[s] - 1 hands on (s >= 1)
+    std::vector<uint32_t> seg_chain;  // two-pass paths: chain cuts, segment s = chains [seg_chain[s], seg_chain[s + 1])
+    std::vector<std::vector<uint32_t>> seg_begin, seg_grid;  // batched path: pass-2 steps of every segment (as ped_begin / ped_grid)
+    uint32_t arena_seg = 0;           // segment whose back-pointers are in the arena
+    DevBuf<uint32_t> d_ckpt, d_bt_state;
     // tile path
     TilePlan tiles;
 
@@ -1148,6 +1198,7 @@ struct whmec_plan {
         d_ped_steps.release(); d_ped_vals.release(); d_chain_len.release(); d_ped_args.release();
         d_in_vec.release(); d_matrix.release(); d_bt_exits.release(); d_bt_entries.release();
         d_chain_rows.release(); d_chain_in.release(); d_chain_out.release();
+        d_ckpt.release(); d_bt_state.release();
         tiles.release(stream);
         if (graph_exec) cudaGraphExecDestroy(graph_exec);
         StreamSet set{stream, ev0, ev1, evh0, evh1};
@@ -1170,7 +1221,9 @@ void keep_host_memory() {
     mallopt(M_TRIM_THRESHOLD, 1 << 30);
 }
 
-int plan_create_impl(const whmec_problem *p, int device, whmec_plan *pl, std::string &msg, int segment = 0) {
+// bounded_t1: a single individual whose back-pointers exceed the free HBM takes the memory-bounded sweep (solve_impl, once no
+// group of chains fits) instead of being refused
+int plan_create_impl(const whmec_problem *p, int device, whmec_plan *pl, std::string &msg, int segment = 0, bool bounded_t1 = false) {
     keep_host_memory();
     // the packer's upload arrays come from page-locked blocks, which belong to a CUDA context: select the device first
     // (a failure here is reported by the checked call below, after the input has been validated as before)
@@ -1258,9 +1311,89 @@ int plan_create_impl(const whmec_problem *p, int device, whmec_plan *pl, std::st
         uint64_t max_ent = 1;
         for (const ColMeta &m : pk.cols) max_ent = std::max<uint64_t>(max_ent, ((uint64_t)1 << m.f) * pk.T);
         uint64_t need = pk.bp_words * 4 + max_ent * (4 * 2 + 8) + pk.fn_delta.size() * 4 + (uint64_t)n * sizeof(ColMeta);
-        if (need + (512ull << 20) > free_b) {
+        constexpr uint64_t RESERVE = 512ull << 20;
+        const uint64_t fixed = need - pk.bp_words * 4;  // everything but the back-pointers
+        const uint64_t hbm_budget = free_b > fixed + RESERVE ? free_b - fixed - RESERVE : 0;
+        // WHMEC_COLUMN_ARENA_BUDGET=bytes (test hook): back-pointers beyond it take the memory-bounded sweep; the budget is the arena's,
+        // checkpoints come on top (as with WHMEC_TILE_ARENA_BUDGET).  Without it the budget is the free HBM and covers both.
+        uint64_t hook = 0;
+        if (const char *e = std::getenv("WHMEC_COLUMN_ARENA_BUDGET")) hook = std::max<uint64_t>(8, std::strtoull(e, nullptr, 10));
+        const bool over_hbm = need + RESERVE > free_b, over_hook = hook && pk.bp_words * 4 > hook;
+        // single individuals: solve_impl first solves groups of chains one after another (grouped.h); the bounded sweep is for
+        // what no group size fits (bounded_t1)
+        const bool bounded = !segment && (over_hook || (over_hbm && (pk.T > 1 || bounded_t1)));
+        if (over_hbm && !bounded) {
             msg = "back-pointer storage exceeds the free HBM of this device";
             return WHMEC_ERR_UNSUPPORTED;
+        }
+        // which sweep: pedigrees with several chains take a two-pass sweep (fused trio kernel or batched), the rest the column sweep
+        const char *seq = std::getenv("WHMEC_PED_SEQUENTIAL");
+        const uint32_t C = (uint32_t)pk.chain_begin.size() - 1;
+        // one trio, shapes of ped_fused.h: one block per chain with the projection in shared memory (3 launches)
+        bool fused_ok = false;
+        {
+            const char *pf = std::getenv("WHMEC_PED_FUSED");
+            fused_ok = !(pf && pf[0] == '0') && pk.T == PF_T && (C >= 2 || segment) && pk.safe31 && !(seq && seq[0] == '1' && !segment);
+            for (uint32_t k = 0; k < n && fused_ok; ++k) fused_ok = pf_column_ok(pk.cols[k], pk.fn_group.data() + pk.cols[k].grp_off);
+        }
+        // batched sweep: the batch buffers (values + argmins of every (chain, unit vector) instance) count against the free HBM as well
+        const uint64_t slots = (uint64_t)C * pk.T + C, batch_bytes = slots * 2 * max_ent * 5;
+        auto batch_ok = [&](uint64_t arena_bytes) {
+            return pk.T > 1 && (C >= 2 || segment) && pk.safe31 && !(seq && seq[0] == '1' && !segment) && slots * 2 * max_ent * 4 < (8ull << 30) &&
+                   (uint64_t)C * pk.T <= 65535 && fixed + arena_bytes + batch_bytes + RESERVE <= free_b;
+        };
+        uint64_t arena_words = pk.bp_words, ckpt_words = 0;
+        bool two_pass = true;  // (resident: whatever the conditions above allow)
+        if (bounded) {
+            std::vector<uint64_t> off(n + 1);
+            for (uint32_t k = 0; k < n; ++k) off[k] = pk.cols[k].bp_off;
+            off[n] = pk.bp_words;
+            // two-pass paths: segments of whole chains, after pass 1 every chain's input is known (no checkpoints)
+            two_pass = false;
+            if (fused_ok || batch_ok(0)) {
+                const uint64_t b2 = over_hook ? hook : fused_ok ? hbm_budget : (hbm_budget > batch_bytes ? hbm_budget - batch_bytes : 0);
+                two_pass = cut_chain_segments(pk.chain_begin, off, b2 / 4, pl->seg_chain, arena_words) && (fused_ok || batch_ok(arena_words * 4));
+            }
+            if (two_pass) {
+                for (size_t sg = 0; sg + 1 < pl->seg_chain.size(); ++sg) {
+                    const uint32_t k0 = pk.chain_begin[pl->seg_chain[sg]], k1 = pk.chain_begin[pl->seg_chain[sg + 1]];
+                    for (uint32_t k = k0; k < k1; ++k) pk.cols[k].bp_off -= off[k0];
+                }
+            } else {  // a chain alone exceeds the budget, or no two-pass sweep: column sweep with checkpoints
+                pl->seg_chain.clear();
+                fused_ok = false;
+                std::vector<uint64_t> ck(n);
+                uint64_t widest = 0, widest_ck = 0;
+                for (uint32_t k = 0; k < n; ++k) {
+                    ck[k] = ((uint64_t)1 << pk.cols[k].f) * pk.T;
+                    widest = std::max(widest, off[k + 1] - off[k]);
+                    widest_ck = std::max(widest_ck, ck[k]);
+                }
+                const bool fits = over_hook ? cut_column_segments(off, {}, hook / 4, pl->seg_col, arena_words, ckpt_words) &&
+                                                  fixed + 4 * (arena_words + ckpt_words) + RESERVE <= free_b
+                                            : cut_column_segments(off, ck, hbm_budget / 4, pl->seg_col, arena_words, ckpt_words);
+                if (!fits) {
+                    msg = over_hook ? "memory-bounded sweep: an arena of " + std::to_string(hook) + " bytes holds no segment; it needs at least " +
+                                          std::to_string(4 * widest) + " bytes (the widest column's back-pointers), checkpoints on top"
+                                    : "memory-bounded sweep: " + std::to_string(hbm_budget) + " bytes of free HBM hold no segment; it needs at least " +
+                                          std::to_string(4 * (widest + widest_ck)) + " bytes (the widest column's back-pointers and the largest checkpoint)";
+                    return WHMEC_ERR_UNSUPPORTED;
+                }
+                if (over_hook)
+                    for (size_t sg = 1; sg + 1 < pl->seg_col.size(); ++sg) ckpt_words += ck[pl->seg_col[sg] - 1];
+                pl->seg_ckpt.assign(pl->seg_col.size() - 1, 0);
+                uint64_t at = 0;
+                for (size_t sg = 0; sg + 1 < pl->seg_col.size(); ++sg) {
+                    const uint32_t k0 = pl->seg_col[sg], k1 = pl->seg_col[sg + 1];
+                    for (uint32_t k = k0; k < k1; ++k) pk.cols[k].bp_off -= off[k0];
+                    if (sg) {
+                        pl->seg_ckpt[sg] = at;
+                        at += ck[k0 - 1];
+                    }
+                }
+            }
+            pl->bounded = true;
+            pl->stats.backptr_bytes = arena_words * 4;
         }
         if (!pl->d_cols.p) CUDA_TRY(pl->d_cols.alloc(n, pl->stream));  // (already there when the tile planner declined the problem)
         CUDA_TRY(pl->d_fn_c0.alloc(pk.fn_c0.size(), pl->stream));
@@ -1270,7 +1403,12 @@ int plan_create_impl(const whmec_problem *p, int device, whmec_plan *pl, std::st
         CUDA_TRY(pl->d_val[0].alloc(max_ent, pl->stream));
         CUDA_TRY(pl->d_val[1].alloc(max_ent, pl->stream));
         CUDA_TRY(pl->d_keys.alloc(max_ent, pl->stream));
-        CUDA_TRY(pl->d_arena.alloc(pk.bp_words + 1, pl->stream));
+        CUDA_TRY(pl->d_arena.alloc(arena_words + 1, pl->stream));
+        if (pl->bounded) {
+            CUDA_TRY(pl->d_ckpt.alloc(ckpt_words, pl->stream));
+            CUDA_TRY(pl->d_bt_state.alloc(2, pl->stream));
+            pl->arena_seg = (uint32_t)(two_pass ? pl->seg_chain.size() : pl->seg_col.size()) - 2;
+        }
         auto up = [&](void *dst, const void *src, size_t bytes) {
             h2d += bytes;
             return cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, pl->stream);
@@ -1281,16 +1419,6 @@ int plan_create_impl(const whmec_problem *p, int device, whmec_plan *pl, std::st
         CUDA_TRY(up(pl->d_fn_group.p, pk.fn_group.data(), pk.fn_group.size() * 4));
         CUDA_TRY(up(pl->d_chain_begin.p, pk.chain_begin.data(), pk.chain_begin.size() * 4));
         pl->stats.path_kind = 2;
-        // pedigrees with several chains: batched two-pass sweep
-        const char *seq = std::getenv("WHMEC_PED_SEQUENTIAL");
-        const uint32_t C = (uint32_t)pk.chain_begin.size() - 1;
-        // one trio, shapes of ped_fused.h: one block per chain with the projection in shared memory (3 launches)
-        bool fused_ok = false;
-        {
-            const char *pf = std::getenv("WHMEC_PED_FUSED");
-            fused_ok = !(pf && pf[0] == '0') && pk.T == PF_T && (C >= 2 || segment) && pk.safe31 && !(seq && seq[0] == '1' && !segment);
-            for (uint32_t k = 0; k < n && fused_ok; ++k) fused_ok = pf_column_ok(pk.cols[k], pk.fn_group.data() + pk.cols[k].grp_off);
-        }
         if (fused_ok) {
             CUDA_TRY(pl->d_chain_rows.alloc((size_t)C * PF_T, pl->stream));
             CUDA_TRY(pl->d_chain_in.alloc((size_t)C * PF_T, pl->stream));
@@ -1313,19 +1441,12 @@ int plan_create_impl(const whmec_problem *p, int device, whmec_plan *pl, std::st
             pl->use_ped_batch = true;  // two-pass sweep: the backtrace and the optimum read the chains' final values
             pl->d_last_vals = pl->d_chain_out.p + (size_t)(C - 1) * PF_T;
             pl->stats.path_kind = 3;
-        } else if (pk.T > 1 && (C >= 2 || segment) && pk.safe31 && !(seq && seq[0] == '1' && !segment)) {
+        } else if (two_pass && batch_ok(arena_words * 4)) {
             const uint32_t T = pk.T;
-            const uint32_t slots = C * T + C;
-            // the batch buffers (values + argmins of every (chain, unit vector) instance) count against the free HBM as well
-            if ((uint64_t)slots * 2 * max_ent * 4 < (8ull << 30) && (uint64_t)C * T <= 65535 &&
-                need + (uint64_t)slots * 2 * max_ent * 5 + (512ull << 20) <= free_b) {
+            {
                 std::vector<PedStep> steps;
                 std::vector<uint32_t> clen(C);
-                uint32_t maxlen = 0;
-                for (uint32_t c = 0; c < C; ++c) {
-                    clen[c] = pk.chain_begin[c + 1] - pk.chain_begin[c];
-                    maxlen = std::max(maxlen, clen[c]);
-                }
+                for (uint32_t c = 0; c < C; ++c) clen[c] = pk.chain_begin[c + 1] - pk.chain_begin[c];
                 auto blocks_for = [&](const ColMeta &m) -> uint32_t {
                     const uint64_t nent = ((uint64_t)1 << m.f) * T;
                     if (m.d > 7) return (uint32_t)nent;
@@ -1333,19 +1454,19 @@ int plan_create_impl(const whmec_problem *p, int device, whmec_plan *pl, std::st
                     return (uint32_t)((nent + epb - 1) / epb);
                 };
                 pl->ped_multi = T <= MULTI_MAX;
-                for (int pass = 0; pass < 3; ++pass) {
-                    pl->ped_begin[pass].clear();
-                    pl->ped_grid[pass].clear();
-                    if (pass == 2 && !pl->ped_multi) continue;
-                    for (uint32_t st = 0; st < maxlen; ++st) {
-                        pl->ped_begin[pass].push_back((uint32_t)steps.size());
+                // the steps of one pass over chains [c_lo, c_hi) (pass 1 of the memory-bounded sweep: one segment)
+                auto add_steps = [&](int pass, uint32_t c_lo, uint32_t c_hi, std::vector<uint32_t> &begin, std::vector<uint32_t> &grid) {
+                    uint32_t len = 0;
+                    for (uint32_t c = c_lo; c < c_hi; ++c) len = std::max(len, clen[c]);
+                    for (uint32_t st = 0; st < len; ++st) {
+                        begin.push_back((uint32_t)steps.size());
                         uint32_t gmax = 0;
                         // pass 0: chain 0 (true input) and, without the multi-RHS kernel, every (chain, unit vector);
                         // pass 1: chains >= 1 with their true inputs; pass 2: one multi-RHS instance per chain >= 1
                         // with the multi-RHS kernel pass 0 is empty: chain 0 (whose input is known: the first column
                         // of the table ignores it) runs in pass 1 like every other chain
-                        const uint32_t c_begin = (pass == 0 && !pl->ped_multi) ? 0 : (pass == 0 ? C : 0);
-                        const uint32_t c_end = C;
+                        const uint32_t c_begin = (pass == 0 && !pl->ped_multi) ? c_lo : (pass == 0 ? c_hi : c_lo);
+                        const uint32_t c_end = c_hi;
                         for (uint32_t c = c_begin; c < c_end; ++c) {
                             if (clen[c] <= st) continue;
                             const uint32_t kcol = pk.chain_begin[c] + st;
@@ -1371,9 +1492,22 @@ int plan_create_impl(const whmec_problem *p, int device, whmec_plan *pl, std::st
                             }
                             gmax = std::max(gmax, blocks_for(m));
                         }
-                        pl->ped_grid[pass].push_back(gmax);
+                        grid.push_back(gmax);
                     }
-                    pl->ped_begin[pass].push_back((uint32_t)steps.size());
+                    begin.push_back((uint32_t)steps.size());
+                };
+                for (int pass = 0; pass < 3; ++pass) {
+                    pl->ped_begin[pass].clear();
+                    pl->ped_grid[pass].clear();
+                    if (pass == 2 && !pl->ped_multi) continue;
+                    if (pass == 1 && pl->bounded) continue;  // per segment, below
+                    add_steps(pass, 0, C, pl->ped_begin[pass], pl->ped_grid[pass]);
+                }
+                if (pl->bounded) {
+                    const size_t S = pl->seg_chain.size() - 1;
+                    pl->seg_begin.assign(S, {});
+                    pl->seg_grid.assign(S, {});
+                    for (size_t sg = 0; sg < S; ++sg) add_steps(1, pl->seg_chain[sg], pl->seg_chain[sg + 1], pl->seg_begin[sg], pl->seg_grid[sg]);
                 }
                 CUDA_TRY(pl->d_ped_steps.alloc(steps.size(), pl->stream));
                 CUDA_TRY(pl->d_ped_vals.alloc((uint64_t)slots * 2 * max_ent, pl->stream));
@@ -1383,7 +1517,7 @@ int plan_create_impl(const whmec_problem *p, int device, whmec_plan *pl, std::st
                 CUDA_TRY(up(pl->d_chain_len.p, clen.data(), C * 4));
                 CUDA_TRY(cudaStreamSynchronize(pl->stream));  // `steps` and `clen` are stack-local
                 pl->ped_max_ent = max_ent;
-                pl->ped_slots = slots;
+                pl->ped_slots = (uint32_t)slots;
                 pl->use_ped_batch = true;
                 const uint32_t last_slot = C * T + (C - 1);
                 pl->d_last_vals = pl->d_ped_vals.p + ((uint64_t)last_slot * 2 + ((clen[C - 1] - 1) & 1u)) * max_ent;
@@ -1422,8 +1556,8 @@ void read_h2d_time(whmec_plan *pl) {
 }
 
 // One pass of the batched pedigree sweep.  pass 0: unit input vectors, values only (transfer matrices);
-// pass 1: true input vectors, back-pointers written.
-int ped_pass(whmec_plan *pl, int pass, uint32_t &launches, std::string &msg) {
+// pass 1: true input vectors, back-pointers written (seg >= 0: only the chains of that segment of the memory-bounded sweep).
+int ped_pass(whmec_plan *pl, int pass, uint32_t &launches, std::string &msg, int seg = -1) {
     Packed &pk = pl->pk;
     const uint32_t T = pk.T, tb = pk.tb;
     if (pass == 0) {
@@ -1431,11 +1565,13 @@ int ped_pass(whmec_plan *pl, int pass, uint32_t &launches, std::string &msg) {
         ped_init_kernel<<<(unit_slots * T + 255) / 256, 256, 0, pl->stream>>>(pl->d_ped_vals.p, pl->ped_max_ent, T, unit_slots);
         ++launches;
     }
-    const size_t nsteps = pl->ped_grid[pass].size();
+    const std::vector<uint32_t> &begin = seg >= 0 ? pl->seg_begin[seg] : pl->ped_begin[pass];
+    const std::vector<uint32_t> &grids = seg >= 0 ? pl->seg_grid[seg] : pl->ped_grid[pass];
+    const size_t nsteps = grids.size();
     for (size_t st = 0; st < nsteps; ++st) {
-        const uint32_t b0 = pl->ped_begin[pass][st], b1 = pl->ped_begin[pass][st + 1];
+        const uint32_t b0 = begin[st], b1 = begin[st + 1];
         if (b1 > b0) {
-            dim3 grid(pl->ped_grid[pass][st], b1 - b0);
+            dim3 grid(grids[st], b1 - b0);
             col_batched_kernel<<<grid, 256, 0, pl->stream>>>(pl->d_ped_steps.p + b0, pl->d_ped_vals.p, pl->ped_max_ent, T, tb,
                                                                pl->d_fn_c0.p, pl->d_fn_delta.p, pl->d_fn_group.p, pl->d_arena.p,
                                                                (uint32_t)(st & 1), pl->d_ped_args.p);
@@ -1466,13 +1602,14 @@ int ped_prefix(whmec_plan *pl, const uint32_t *d_in_vec, uint32_t &launches, std
 }
 
 // the fused sweep in pieces: pass 1 (unit input e_0 of every chain, values only), prefix, pass 2 (true inputs, back-pointers)
-PedFusedArgs ped_fused_args(whmec_plan *pl, bool unit) {
+PedFusedArgs ped_fused_args(whmec_plan *pl, bool unit, uint32_t chain0) {
     return PedFusedArgs{pl->d_cols.p, pl->d_chain_begin.p, pl->d_fn_c0.p, pl->d_fn_group.p, pl->d_fn_delta.p, pl->d_arena.p,
-                        pl->d_chain_in.p, unit ? pl->d_chain_rows.p : pl->d_chain_out.p, unit ? 1u : 0u};
+                        pl->d_chain_in.p, unit ? pl->d_chain_rows.p : pl->d_chain_out.p, unit ? 1u : 0u, chain0};
 }
 
-int ped_fused_pass(whmec_plan *pl, bool unit, std::string &msg) {
-    const uint32_t C = (uint32_t)pl->pk.chain_begin.size() - 1;
+// chains [c0, c0 + count); count == 0: all chains
+int ped_fused_pass(whmec_plan *pl, bool unit, std::string &msg, uint32_t c0 = 0, uint32_t count = 0) {
+    const uint32_t C = count ? count : (uint32_t)pl->pk.chain_begin.size() - 1;
     if (pl->ped_cluster > 1) {
         cudaLaunchConfig_t cfg = {};
         cfg.gridDim = dim3(C * pl->ped_cluster);
@@ -1486,9 +1623,9 @@ int ped_fused_pass(whmec_plan *pl, bool unit, std::string &msg) {
         attr[0].val.clusterDim.z = 1;
         cfg.attrs = attr;
         cfg.numAttrs = 1;
-        CUDA_TRY(cudaLaunchKernelEx(&cfg, ped_fused_cluster_kernel, ped_fused_args(pl, unit)));
+        CUDA_TRY(cudaLaunchKernelEx(&cfg, ped_fused_cluster_kernel, ped_fused_args(pl, unit, c0)));
     } else {
-        ped_fused_kernel<<<C, PF_THREADS, PF_SMEM, pl->stream>>>(ped_fused_args(pl, unit));
+        ped_fused_kernel<<<C, PF_THREADS, PF_SMEM, pl->stream>>>(ped_fused_args(pl, unit, c0));
     }
     CUDA_TRY(cudaGetLastError());
     return WHMEC_OK;
@@ -1501,12 +1638,33 @@ int ped_fused_prefix(whmec_plan *pl, const uint32_t *d_in_vec, uint32_t *d_matri
     return WHMEC_OK;
 }
 
-// three launches for the whole table
+// pass 2 of the two-pass sweeps for the chains of segment `seg` of the memory-bounded sweep (their back-pointers -> the arena)
+int ped_segment_pass(whmec_plan *pl, uint32_t seg, uint32_t &launches, std::string &msg) {
+    int rc;
+    if (pl->use_ped_fused) {
+        rc = ped_fused_pass(pl, false, msg, pl->seg_chain[seg], pl->seg_chain[seg + 1] - pl->seg_chain[seg]);
+        ++launches;
+    } else {
+        rc = ped_pass(pl, 1, launches, msg, (int)seg);
+    }
+    pl->arena_seg = seg;
+    return rc;
+}
+
+// three launches for the whole table (memory-bounded: pass 2 for the last segment only, the backtrace sweeps the others)
 int ped_fused_sweep(whmec_plan *pl, std::string &msg) {
     int rc = ped_fused_pass(pl, true, msg);
     if (rc == WHMEC_OK) rc = ped_fused_prefix(pl, nullptr, nullptr, msg);
-    if (rc == WHMEC_OK) rc = ped_fused_pass(pl, false, msg);
-    pl->stats.kernel_launches = 3;
+    uint32_t launches = 2;
+    if (rc == WHMEC_OK) {
+        if (pl->bounded) {
+            rc = ped_segment_pass(pl, (uint32_t)pl->seg_chain.size() - 2, launches, msg);
+        } else {
+            rc = ped_fused_pass(pl, false, msg);
+            ++launches;
+        }
+    }
+    pl->stats.kernel_launches = launches;
     return rc;
 }
 
@@ -1515,58 +1673,84 @@ int ped_batched_sweep(whmec_plan *pl, std::string &msg) {
     uint32_t launches = 0;
     int rc = ped_pass(pl, 0, launches, msg);
     if (rc == WHMEC_OK) rc = ped_prefix(pl, nullptr, launches, msg);
-    if (rc == WHMEC_OK) rc = ped_pass(pl, 1, launches, msg);
+    if (rc == WHMEC_OK) rc = pl->bounded ? ped_segment_pass(pl, (uint32_t)pl->seg_chain.size() - 2, launches, msg) : ped_pass(pl, 1, launches, msg);
     pl->stats.kernel_launches = launches;
     return rc;
 }
 
+// Column k of the column sweep: reads the values of column k - 1 from `prev`, writes its own to `out` and its back-pointers to the
+// arena.  (capture: the stream is being captured into a graph; an error ends the capture.)
+int column_launch(whmec_plan *pl, uint32_t k, const uint32_t *prev, uint32_t *out, bool capture, uint32_t &launches, std::string &msg) {
+    Packed &pk = pl->pk;
+    const uint32_t T = pk.T, tb = pk.tb;
+    const ColMeta &m = pk.cols[k];
+    const uint64_t nent = ((uint64_t)1 << m.f) * T;
+    if (m.d <= 6) {
+        const uint32_t lc = col_lane_bits(m.f + tb, m.d);
+        const uint64_t ent_per_block = 256u >> lc;
+        const unsigned blocks = (unsigned)((nent + ent_per_block - 1) / ent_per_block);
+        col_direct_kernel<<<blocks, 256, 0, pl->stream>>>(m, pk.fn_group[m.grp_off + T], T, tb, pl->d_fn_c0.p, pl->d_fn_delta.p,
+                                                           pl->d_fn_group.p, prev, out, pl->d_arena.p);
+        launches += 1;
+    } else {
+        const uint32_t log_chunks = m.d - 6;
+        if (cudaError_t e = cudaMemsetAsync(pl->d_keys.p, 0xFF, nent * 8, pl->stream); e != cudaSuccess) {
+            if (capture) {  // do not leave the stream in capture mode
+                cudaGraph_t dead = nullptr;
+                cudaStreamEndCapture(pl->stream, &dead);
+                if (dead) cudaGraphDestroy(dead);
+            }
+            msg = std::string("cudaMemsetAsync (column sweep): ") + cudaGetErrorString(e);
+            return WHMEC_ERR_CUDA;
+        }
+        const uint64_t threads = nent << log_chunks;
+        const unsigned blocks = (unsigned)((threads + 255) / 256);
+        col_chunk_kernel<<<blocks, 256, 0, pl->stream>>>(m, pk.fn_group[m.grp_off + T], T, tb, pl->d_fn_c0.p, pl->d_fn_delta.p,
+                                                          pl->d_fn_group.p, prev, log_chunks, pl->d_keys.p);
+        col_finalize_kernel<<<(unsigned)((nent + 255) / 256), 256, 0, pl->stream>>>(pl->d_cols.p, k, T, tb, pl->d_keys.p,
+                                                                                      out, pl->d_arena.p);
+        launches += 2;
+    }
+    return WHMEC_OK;
+}
+
 // The column path issues one (small) kernel per column; a sweep of the same plan is replayed from a
-// CUDA graph from the second time on (launch-bound inner loop, captured once).
+// CUDA graph from the second time on (launch-bound inner loop, captured once).  Memory-bounded: the values in front of every
+// segment but the first are copied to its checkpoint, and the arena ends up holding the last segment's back-pointers.
 int column_sweep(whmec_plan *pl, std::string &msg) {
     Packed &pk = pl->pk;
-    const uint32_t n = pk.n, T = pk.T, tb = pk.tb;
+    const uint32_t n = pk.n, T = pk.T;
     if (pl->graph_exec) {
         CUDA_TRY(cudaGraphLaunch(pl->graph_exec, pl->stream));
+        pl->arena_seg = pl->bounded ? (uint32_t)pl->seg_col.size() - 2 : 0;
         return WHMEC_OK;
     }
     const bool capture = pl->sweeps_done >= 1 && n >= 64;
     if (capture) CUDA_TRY(cudaStreamBeginCapture(pl->stream, cudaStreamCaptureModeThreadLocal));
     uint32_t launches = 0;
     uint32_t curb = 0;
+    size_t next_cut = 1;  // bounded: the next segment whose checkpoint is due
     for (uint32_t k = 0; k < n; ++k) {
-        const ColMeta &m = pk.cols[k];
-        const uint64_t nent = ((uint64_t)1 << m.f) * T;
-        const uint32_t *prev = pl->d_val[curb ^ 1].p;
-        uint32_t *out = pl->d_val[curb].p;
-        if (m.d <= 6) {
-            const uint32_t lc = col_lane_bits(m.f + tb, m.d);
-            const uint64_t ent_per_block = 256u >> lc;
-            const unsigned blocks = (unsigned)((nent + ent_per_block - 1) / ent_per_block);
-            col_direct_kernel<<<blocks, 256, 0, pl->stream>>>(m, pk.fn_group[m.grp_off + T], T, tb, pl->d_fn_c0.p, pl->d_fn_delta.p,
-                                                               pl->d_fn_group.p, prev, out, pl->d_arena.p);
-            launches += 1;
-        } else {
-            const uint32_t log_chunks = m.d - 6;
-            if (cudaError_t e = cudaMemsetAsync(pl->d_keys.p, 0xFF, nent * 8, pl->stream); e != cudaSuccess) {
-                if (capture) {  // do not leave the stream in capture mode
+        int rc = column_launch(pl, k, pl->d_val[curb ^ 1].p, pl->d_val[curb].p, capture, launches, msg);
+        if (rc != WHMEC_OK) return rc;
+        if (pl->bounded && next_cut + 1 < pl->seg_col.size() && k + 1 == pl->seg_col[next_cut]) {
+            const size_t bytes = ((size_t)1 << pk.cols[k].f) * T * 4;
+            cudaError_t e = cudaMemcpyAsync(pl->d_ckpt.p + pl->seg_ckpt[next_cut], pl->d_val[curb].p, bytes, cudaMemcpyDeviceToDevice, pl->stream);
+            if (e != cudaSuccess) {
+                if (capture) {
                     cudaGraph_t dead = nullptr;
                     cudaStreamEndCapture(pl->stream, &dead);
                     if (dead) cudaGraphDestroy(dead);
                 }
-                msg = std::string("cudaMemsetAsync (column sweep): ") + cudaGetErrorString(e);
+                msg = std::string("cudaMemcpyAsync (checkpoint): ") + cudaGetErrorString(e);
                 return WHMEC_ERR_CUDA;
             }
-            const uint64_t threads = nent << log_chunks;
-            const unsigned blocks = (unsigned)((threads + 255) / 256);
-            col_chunk_kernel<<<blocks, 256, 0, pl->stream>>>(m, pk.fn_group[m.grp_off + T], T, tb, pl->d_fn_c0.p, pl->d_fn_delta.p,
-                                                              pl->d_fn_group.p, prev, log_chunks, pl->d_keys.p);
-            col_finalize_kernel<<<(unsigned)((nent + 255) / 256), 256, 0, pl->stream>>>(pl->d_cols.p, k, T, tb, pl->d_keys.p,
-                                                                                          out, pl->d_arena.p);
-            launches += 2;
+            ++next_cut;
         }
         curb ^= 1;
     }
     pl->last_buf = curb ^ 1;
+    if (pl->bounded) pl->arena_seg = (uint32_t)pl->seg_col.size() - 2;
     pl->stats.kernel_launches = launches;
     if (capture) {
         cudaGraph_t graph = nullptr;
@@ -1640,6 +1824,51 @@ int pedigree_backtrace(whmec_plan *pl, int entry, std::string &msg) {
     return WHMEC_OK;
 }
 
+// Backtrace of the memory-bounded sweep, segment by segment from the right; every segment but the one whose back-pointers the
+// sweep left in the arena is swept again first (launches counted in kernel_launches).
+//   two-pass paths: pass 2 for the segment's chains from their true inputs (known since pass 1), then the three backtrace kernels
+//     on its chains; the value the segment's first chain hands to its predecessor stays on the device (d_bt_state[0]).
+//   column sweep: the segment's columns from its checkpoint, then one warp walks them (bt_segment_kernel).
+int bounded_backtrace(whmec_plan *pl, std::string &msg) {
+    const Packed &pk = pl->pk;
+    uint32_t launches = 0;
+    int rc = WHMEC_OK;
+    if (!pl->seg_chain.empty()) {
+        const uint32_t S = (uint32_t)pl->seg_chain.size() - 1;
+        for (uint32_t sg = S; sg-- > 0;) {
+            if (pl->arena_seg != sg && (rc = ped_segment_pass(pl, sg, launches, msg)) != WHMEC_OK) return rc;
+            const uint32_t c0 = pl->seg_chain[sg];
+            BtArgs a = bt_args(pl, sg + 1 == S ? -1 : 0);
+            a.chain_begin += c0;
+            a.n_chains = pl->seg_chain[sg + 1] - c0;
+            bt_exits_kernel<<<a.n_chains * a.T, 32, 0, pl->stream>>>(a, pl->d_bt_exits.p);
+            bt_entries_kernel<<<1, 32, 0, pl->stream>>>(a, pl->d_bt_exits.p, pl->d_bt_entries.p, nullptr, pl->d_bt_state.p);
+            bt_paths_kernel<<<a.n_chains, 32, 0, pl->stream>>>(a, pl->d_bt_entries.p, pl->d_path_index.p, pl->d_path_tv.p,
+                                                                sg + 1 == S ? pl->d_result.p : nullptr);
+            CUDA_TRY(cudaGetLastError());
+        }
+    } else {
+        const uint32_t S = (uint32_t)pl->seg_col.size() - 1;
+        const BtView v{pl->d_cols.p, pl->d_arena.p, pk.T, pk.tb};
+        for (uint32_t sg = S; sg-- > 0;) {
+            const uint32_t k0 = pl->seg_col[sg], k1 = pl->seg_col[sg + 1];
+            if (pl->arena_seg != sg) {
+                for (uint32_t k = k0; k < k1; ++k) {
+                    const uint32_t *prev = k == k0 && sg ? pl->d_ckpt.p + pl->seg_ckpt[sg] : pl->d_val[(k & 1) ^ 1].p;
+                    if ((rc = column_launch(pl, k, prev, pl->d_val[k & 1].p, false, launches, msg)) != WHMEC_OK) return rc;
+                }
+                pl->arena_seg = sg;
+            }
+            // (the last segment: its last column's values are still where the sweep left them -- or were re-swept just now)
+            bt_segment_kernel<<<1, 32, 0, pl->stream>>>(v, k1 - 1, k0, sg + 1 == S ? pl->d_val[pl->last_buf].p : nullptr, pl->d_bt_state.p,
+                                                         pl->d_path_index.p, pl->d_path_tv.p, pl->d_result.p);
+            CUDA_TRY(cudaGetLastError());
+        }
+    }
+    pl->stats.kernel_launches += launches;
+    return WHMEC_OK;
+}
+
 int plan_finish_impl(whmec_plan *pl, whmec_solution *s, std::string &msg, int entry = -1) {
     Packed &pk = pl->pk;
     const uint32_t n = pk.n;
@@ -1670,7 +1899,10 @@ int plan_finish_impl(whmec_plan *pl, whmec_solution *s, std::string &msg, int en
     } else {
         const uint32_t n_chains = (uint32_t)pk.chain_begin.size() - 1;
         const uint32_t *last_vals = pl->use_ped_batch ? pl->d_last_vals : pl->d_val[pl->last_buf].p;
-        if (pk.T == 1) {
+        if (pl->bounded) {
+            int rc = bounded_backtrace(pl, msg);
+            if (rc != WHMEC_OK) return rc;
+        } else if (pk.T == 1) {
             backtrace_kernel<<<(n_chains + 63) / 64, 64, 0, pl->stream>>>(pl->d_cols.p, pl->d_arena.p, pl->d_chain_begin.p, n_chains, n,
                                                                            last_vals, pl->d_path_index.p, pl->d_path_tv.p, pl->d_result.p);
         } else {
@@ -1881,12 +2113,12 @@ int whmec_device_count(void) {
     return n;
 }
 
-int whmec_plan_create(const whmec_problem *p, int device, whmec_plan **out, char *err, size_t errlen) {
+static int plan_create_guarded(const whmec_problem *p, int device, whmec_plan **out, char *err, size_t errlen, bool bounded_t1) {
     return guarded(err, errlen, [&]() -> int {
         std::string msg;
         *out = nullptr;
         std::unique_ptr<whmec_plan> pl(new whmec_plan());  // released (device buffers too) if anything below throws
-        const int rc = plan_create_impl(p, device, pl.get(), msg);
+        const int rc = plan_create_impl(p, device, pl.get(), msg, 0, bounded_t1);
         if (rc != WHMEC_OK) {
             set_err(err, errlen, msg);
             return rc;
@@ -1894,6 +2126,10 @@ int whmec_plan_create(const whmec_problem *p, int device, whmec_plan **out, char
         *out = pl.release();
         return WHMEC_OK;
     });
+}
+
+int whmec_plan_create(const whmec_problem *p, int device, whmec_plan **out, char *err, size_t errlen) {
+    return plan_create_guarded(p, device, out, err, errlen, false);
 }
 
 int whmec_plan_sweep(whmec_plan *plan, char *err, size_t errlen) {
@@ -2016,6 +2252,8 @@ static int solve_impl(const whmec_problem *p, whmec_solution *s, int device, whm
                 return WHMEC_OK;
             }
         }
+        // no group fits (one chain alone is too large): the memory-bounded sweep of the whole table
+        rc = plan_create_guarded(p, device, &pl, err, errlen, true);
     }
     if (rc != WHMEC_OK) return rc;
     const auto t1 = clk::now();

@@ -176,6 +176,64 @@ def trio(
     )
 
 
+def nuclear_family(
+    n: int,
+    children: int = 1,
+    c_per_sample: int = 5,
+    block_len: int = 500,
+    err: float = 0.05,
+    seed: int = 0,
+    recomb_every: int = 5000,
+    max_phred: int = 40,
+) -> FlatProblem:
+    """Father, mother and `children` children (indices 0, 1, 2 ..; one trio per child, T = 4^children), shaped like `trio`:
+    `c_per_sample` reads per sample per column.  (`trio` stays as it is: cfg5's inputs must not change.)"""
+    rng = np.random.Generator(np.random.PCG64(seed))
+    n_ind = 2 + children
+    f1, l1 = _window_spans(n, c_per_sample, 1, block_len)
+    m = f1.size
+    first = np.concatenate([f1] * n_ind)
+    last = np.concatenate([l1] * n_ind)
+    ind = np.repeat(np.arange(n_ind, dtype=np.uint32), m)
+    start_key = np.concatenate([np.arange(m)] * n_ind)
+    order = np.lexsort((ind, start_key, first))  # ReadSet order: by first column, then deterministic
+    first, last, ind = first[order], last[order], ind[order]
+    off, cols = _csr_from_spans(first, last)
+    lens = (last - first + 1).astype(np.int64)
+    nnz = cols.size
+    hap = rng.integers(0, 2, (2, 2, n), dtype=np.uint8)  # [parent][haplotype][col]
+    kids = []
+    for _ in range(children):  # each child inherits one haplotype per parent with rare recombination
+        sel = np.zeros((2, n), np.uint8)
+        for par in range(2):
+            brk = rng.random(n) < (1.0 / max(recomb_every, 1))
+            sel[par] = (int(rng.integers(0, 2)) + np.cumsum(brk)) & 1
+        kids.append(np.stack([np.where(sel[0] == 0, hap[0, 0], hap[0, 1]), np.where(sel[1] == 0, hap[1, 0], hap[1, 1])]))
+    haps = np.stack([hap[0], hap[1]] + kids)  # [ind][haplotype][col]
+    gt = (haps[:, 0, :] + haps[:, 1, :]).astype(np.uint8)
+    read_hap = rng.integers(0, 2, first.size, dtype=np.uint8)
+    flips = (rng.random(nnz) < err).astype(np.uint8)
+    rid = np.repeat(np.arange(first.size), lens)
+    allele = haps[ind[rid], read_hap[rid], cols] ^ flips
+    phred = rng.integers(1, max_phred + 1, nnz, dtype=np.uint32)
+    recomb = np.full(n, 49, np.uint32)
+    if n:
+        recomb[0] = 0
+    return FlatProblem(
+        positions=(np.arange(n, dtype=np.uint32) + 1) * 1000,
+        read_off=off,
+        ent_col=cols,
+        ent_allele=allele.astype(np.uint8),
+        ent_phred=phred,
+        read_ind=ind,
+        recombcost=recomb,
+        n_ind=n_ind,
+        trios=np.array([[0, 1, 2 + i] for i in range(children)], np.uint32).reshape(-1),
+        distrust=False,
+        gt=gt,
+    )
+
+
 def config(name: str, n: Optional[int] = None) -> FlatProblem:
     """The four GPU configurations of BASELINE.json (cfg2..cfg5) and the ragged variant of cfg3; `n` overrides the column count."""
     if name == "cfg2":
