@@ -138,8 +138,13 @@ int whmec_solve(const whmec_problem *p, whmec_solution *s, int device, whmec_sta
  * likelihoods (caller-allocated, [n_ind][n_cols][3] doubles) receives get_genotype_likelihoods(individual, column)
  * for every individual (pedigree index order) and column.  Floating point: the reference computes in 80-bit long
  * double with running-sum scaling, the device in double with max scaling; the normalised likelihoods agree to
- * ~1e-13 (the reference's own tests compare with 1e-9, whatshap/testhelpers.py:11-15).  st->backptr_bytes reports
- * the bytes of backward tables kept in HBM, st->sweep_ms the device time of both passes. */
+ * ~1e-13 (the reference's own tests compare with 1e-9, whatshap/testhelpers.py:11-15).  A table whose backward
+ * tables do not fit the free HBM is cut into segments that share one arena and is swept backward again from
+ * checkpoints (same likelihoods, more launches).  Besides pedigrees beyond GL_MAX_*, WHMEC_ERR_UNSUPPORTED only when
+ * the fixed per-column arrays do not fit, or when not even one column per segment does; the message then says "needs at least N bytes" (for backward
+ * tables, checkpoints and projection buffers).  st->backptr_bytes reports the bytes of backward tables kept in HBM (with
+ * a table cut into segments: the largest store allocated, arena + checkpoints), st->sweep_ms the device time of both
+ * passes, st->kernel_launches includes the repeated backward sweeps. */
 int whmec_genotype(const whmec_problem *p, double *likelihoods, int device, whmec_stats *st_or_null, char *err, size_t errlen);
 
 /* Per-column genotype priors of one sample's reads, the step `whatshap genotype` runs before the DP above

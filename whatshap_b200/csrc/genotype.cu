@@ -7,12 +7,15 @@
 // Per step: backward pass  gl_backward_kernel + gl_scale_kernel,  forward pass  gl_forward_kernel + gl_scale_kernel;
 // one launch advances every table of a group by one column (gl_schedule, gl_pack.cpp): for a single individual the
 // DP-independent chains are tables of their own, so the launch count is 4 x (longest chain), not 4 x (columns).
-// The backward tables of all columns of a group stay in HBM (the reference keeps every sqrt(n)-th and recomputes,
-// genotypedptable.cpp:139-166,326-343).
+// The backward tables of all columns of a group stay in HBM.  A table whose backward tables do not fit runs alone in
+// memory-bounded mode (gl_bounded, DESIGN §4.5): its columns are cut into segments that share one arena, and every
+// segment but the first is swept backward again from a checkpoint before its forward steps (the reference keeps every
+// sqrt(n)-th column and recomputes, genotypedptable.cpp:139-166,326-343).
 #include <cuda_runtime.h>
 
 #include <algorithm>
 #include <chrono>
+#include <cstdlib>
 #include <cstring>
 #include <string>
 #include <vector>
@@ -145,27 +148,24 @@ int genotype_impl(const whmec_problem *p, double *likelihoods, int device, whmec
         msg = "genotyping: problem exceeds the free HBM of this device";
         return WHMEC_ERR_UNSUPPORTED;
     }
-    const uint64_t budget = (free_b - fixed) / 8;  // doubles available for backward tables + projection buffers
-    std::vector<uint32_t> group_begin;
-    if (!gl_groups(g, T, budget, group_begin)) {
-        msg = "genotyping: the backward tables of one chain exceed the free HBM of this device";
-        return WHMEC_ERR_UNSUPPORTED;
-    }
-    // launch schedules of the groups (one launch advances every table of a group by one column)
-    std::vector<GlSchedule> schedules(group_begin.size() - 1);
-    uint64_t max_group = 0, max_pool = 1, max_steps = 1;
-    for (size_t q = 0; q + 1 < group_begin.size(); ++q) {
-        gl_schedule(g, T, group_begin[q], group_begin[q + 1], schedules[q]);
-        max_group = std::max(max_group, schedules[q].beta_doubles);
-        max_pool = std::max(max_pool, schedules[q].f_pool_doubles);
-        max_steps = std::max<uint64_t>(max_steps, schedules[q].steps.size());
-    }
-    if ((max_group + max_pool) > budget) {  // the two projection buffers per table count too
-        msg = "genotyping: backward tables and projection buffers exceed the free HBM of this device";
-        return WHMEC_ERR_UNSUPPORTED;
+    uint64_t budget = (free_b - fixed) / 8;  // doubles available for backward tables + projection buffers
+    // WHMEC_GENOTYPE_ARENA_BUDGET=bytes (test hook): the budget for backward tables, checkpoints and projection buffers
+    if (const char *e = std::getenv("WHMEC_GENOTYPE_ARENA_BUDGET")) budget = std::min<uint64_t>(budget, std::strtoull(e, nullptr, 10) / 8);
+    // groups of tables on launch schedules (one launch advances every table of a group by one column); a table whose
+    // backward tables do not fit runs alone in memory-bounded mode (gl_bounded)
+    std::vector<GlUnit> units;
+    rc = gl_plan(g, T, budget, units, msg);
+    if (rc != WHMEC_OK) return rc;
+    uint64_t max_work = 1, max_steps = 1, max_store = 0;  // max_store: the largest backward store of a unit (doubles)
+    bool bounded = false;
+    for (const GlUnit &u : units) {
+        max_work = std::max(max_work, u.work_doubles);
+        max_steps = std::max<uint64_t>(max_steps, u.bounded ? u.bd.steps.size() : u.sc.steps.size());
+        max_store = std::max(max_store, u.bounded ? u.bd.arena_doubles + u.bd.ckpt_doubles : u.sc.beta_doubles);
+        bounded = bounded || u.bounded;
     }
     GlCol *d_cols = nullptr;
-    double *d_eps = nullptr, *d_trans = nullptr, *d_q = nullptr, *d_beta = nullptr, *d_F = nullptr, *d_acc = nullptr;
+    double *d_eps = nullptr, *d_trans = nullptr, *d_q = nullptr, *d_work = nullptr, *d_acc = nullptr;
     GlStep *d_steps = nullptr;
     uint8_t *d_allele = nullptr, *d_ind = nullptr;
     int8_t *d_h2p = nullptr;
@@ -176,8 +176,7 @@ int genotype_impl(const whmec_problem *p, double *likelihoods, int device, whmec
     CUDA_TRY(B.alloc(&d_h2p, pk.h2p.size()));
     CUDA_TRY(B.alloc(&d_trans, g.trans.size()));
     CUDA_TRY(B.alloc(&d_q, g.q.size()));
-    CUDA_TRY(B.alloc(&d_beta, max_group + 1));
-    CUDA_TRY(B.alloc(&d_F, max_pool));
+    CUDA_TRY(B.alloc(&d_work, max_work));  // per unit: its backward store, then its projection buffers
     CUDA_TRY(B.alloc(&d_steps, max_steps));
     CUDA_TRY(B.alloc(&d_acc, (size_t)n * n_ind * 3));
     uint64_t h2d = 0;
@@ -201,9 +200,33 @@ int genotype_impl(const whmec_problem *p, double *likelihoods, int device, whmec
     CUDA_TRY(cudaEventRecord(ev0, s));
     uint32_t launches = 0;
     constexpr uint32_t MAX_GRID_Y = 65535;
-    for (size_t q = 0; q + 1 < group_begin.size(); ++q) {
-        const GlSchedule &sc = schedules[q];
-        if (q > 0) CUDA_TRY(cudaStreamSynchronize(s));  // the step list of the previous group is still being read
+    for (size_t q = 0; q < units.size(); ++q) {
+        if (q > 0) CUDA_TRY(cudaStreamSynchronize(s));  // the step list of the previous unit is still being read
+        if (units[q].bounded) {
+            const GlBounded &bd = units[q].bd;
+            const uint64_t store = bd.arena_doubles + bd.ckpt_doubles;
+            double *d_beta = d_work, *d_F = d_work + store;
+            CUDA_TRY(up(d_steps, bd.steps.data(), bd.steps.size() * sizeof(GlStep)));
+            CUDA_TRY(cudaMemsetAsync(d_work, 0, (store + bd.f_pool_doubles) * 8, s));
+            auto blocks = [&](uint32_t e) { return (unsigned)((((uint64_t)1 << bd.steps[e].cells_log2) + GL_THREADS - 1) / GL_THREADS); };
+            for (const GlSweep &sw : bd.sweeps) {
+                if (sw.clear) CUDA_TRY(cudaMemsetAsync(d_beta, 0, sw.clear * 8, s));
+                if (sw.copy_n) CUDA_TRY(cudaMemcpyAsync(d_beta + sw.copy_dst, d_beta + sw.copy_src, sw.copy_n * 8, cudaMemcpyDeviceToDevice, s));
+                for (uint32_t e = sw.bwd_begin; e < sw.bwd_end; ++e) {
+                    gl_backward_kernel<<<blocks(e), GL_THREADS, 0, s>>>(v, d_steps + e, d_beta, sw.beta_base);
+                    gl_scale_kernel<<<1, 1024, 0, s>>>(d_steps + e, d_beta);
+                    launches += 2;
+                }
+                for (uint32_t e = sw.fwd_begin; e < sw.fwd_end; ++e) {
+                    gl_forward_kernel<<<blocks(e), GL_THREADS, 0, s>>>(v, d_steps + e, d_F, d_beta, sw.beta_base, d_acc);
+                    gl_scale_kernel<<<1, 1024, 0, s>>>(d_steps + e, d_F);
+                    launches += 2;
+                }
+            }
+            continue;
+        }
+        const GlSchedule &sc = units[q].sc;
+        double *d_beta = d_work, *d_F = d_work + sc.beta_doubles + 1;
         CUDA_TRY(up(d_steps, sc.steps.data(), sc.steps.size() * sizeof(GlStep)));
         CUDA_TRY(cudaMemsetAsync(d_beta, 0, (sc.beta_doubles + 1) * 8, s));
         CUDA_TRY(cudaMemsetAsync(d_F, 0, sc.f_pool_doubles * 8, s));
@@ -242,7 +265,9 @@ int genotype_impl(const whmec_problem *p, double *likelihoods, int device, whmec
         st->sweep_ms = ms;
         st->h2d_bytes = h2d;
         st->d2h_bytes = acc.size() * 8;
-        st->backptr_bytes = g.beta_doubles * 8;  // here: bytes of backward tables kept in HBM
+        // here: bytes of backward tables kept in HBM; with a table in bounded mode, the largest store allocated for them
+        // (arena + checkpoints of a bounded table, the backward tables of a group)
+        st->backptr_bytes = bounded ? max_store * 8 : g.beta_doubles * 8;
         st->path_kind = 4;
     }
     return WHMEC_OK;

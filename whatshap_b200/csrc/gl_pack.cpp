@@ -10,6 +10,8 @@
 #include <cstring>
 #include <map>
 
+#include "bounded.h"
+
 namespace whmec {
 
 namespace {
@@ -159,8 +161,9 @@ void gl_schedule(const GlPacked &g, uint32_t T, uint32_t lo, uint32_t hi, GlSche
     out.fwd_begin.push_back((uint32_t)out.steps.size());
 }
 
-bool gl_groups(const GlPacked &g, uint32_t T, uint64_t budget, std::vector<uint32_t> &begin) {
+void gl_groups_split(const GlPacked &g, uint32_t T, uint64_t budget, std::vector<uint32_t> &begin, std::vector<uint8_t> &alone) {
     begin.assign(1, 0);
+    alone.clear();
     const uint32_t n = (uint32_t)g.cols.size();
     uint64_t run = 0, table = 0, widest = 1;
     uint32_t table_begin = 0;
@@ -172,18 +175,151 @@ bool gl_groups(const GlPacked &g, uint32_t T, uint64_t budget, std::vector<uint3
             continue;
         }
         const uint64_t cost = table + 2 * widest;  // a table ends here: its backward tables and its two projection buffers
-        if (cost > budget) return false;
-        if (run + cost > budget) {  // close the group before this table
-            begin.push_back(table_begin);
+        if (cost > budget) {  // a group of its own: close the open group (if any) before it and start a new one after it
+            if (table_begin > begin.back()) {
+                begin.push_back(table_begin);
+                alone.push_back(0);
+            }
+            begin.push_back(k + 1);
+            alone.push_back(1);
             run = 0;
+        } else {
+            if (run + cost > budget) {  // close the group before this table
+                begin.push_back(table_begin);
+                alone.push_back(0);
+                run = 0;
+            }
+            run += cost;
         }
-        run += cost;
         table_begin = k + 1;
         table = 0;
         widest = 1;
     }
-    begin.push_back(n);
+    if (begin.back() < n) {
+        begin.push_back(n);
+        alone.push_back(0);
+    }
+}
+
+bool gl_groups(const GlPacked &g, uint32_t T, uint64_t budget, std::vector<uint32_t> &begin) {
+    std::vector<uint8_t> alone;
+    gl_groups_split(g, T, budget, begin, alone);
+    return std::find(alone.begin(), alone.end(), 1) == alone.end();
+}
+
+bool gl_bounded(const GlPacked &g, uint32_t T, uint32_t lo, uint32_t hi, uint64_t budget, GlBounded &out) {
+    out = GlBounded();
+    const uint32_t m = hi - lo;
+    auto own = [&](uint32_t k) { return g.cols[k].last ? 0 : ((uint64_t)1 << g.cols[k].f) * T; };  // doubles of B_k
+    uint64_t f_size = 1;
+    for (uint32_t k = lo; k < hi; ++k) f_size = std::max(f_size, own(k));
+    out.f_pool_doubles = 2 * f_size;
+    if (budget <= out.f_pool_doubles) return false;
+    // mirrored order: column j is column hi - 1 - j.  A mirrored segment that starts at j + 1 is a segment that ends at column
+    // hi - 2 - j; its checkpoint is B_{hi - 2 - j}.
+    std::vector<uint64_t> off(m + 1, 0), ck(m, 0);
+    for (uint32_t j = 0; j < m; ++j) {
+        off[j + 1] = off[j] + own(hi - 1 - j);
+        if (j + 1 < m) ck[j] = own(hi - 2 - j);
+    }
+    std::vector<uint32_t> mcuts;
+    if (!cut_column_segments(off, ck, budget - out.f_pool_doubles, mcuts, out.arena_doubles, out.ckpt_doubles)) return false;
+    for (size_t c = mcuts.size(); c-- > 0;) out.cuts.push_back(hi - mcuts[c]);
+    const uint32_t S = (uint32_t)out.cuts.size() - 1;
+    const std::vector<uint32_t> &c = out.cuts;
+    const uint64_t A = out.arena_doubles;
+    std::vector<uint64_t> ckpt(S, 0);  // store offset of segment s's checkpoint (s < S - 1)
+    uint64_t at = 0;
+    for (uint32_t s = 0; s + 1 < S; ++s) {
+        ckpt[s] = A + at;
+        at += own(c[s + 1] - 1);
+    }
+    auto beta_off = [&](uint32_t k) { return g.cols[k].beta_off; };
+    auto backward = [&](uint32_t k, uint64_t dst) {  // column k reads B_k, adds into B_{k-1} at dst
+        GlStep st{};
+        st.k = k;
+        st.cells_log2 = g.cols[k].a;
+        st.cur_off = dst;
+        st.n_scale = own(k - 1);
+        out.steps.push_back(st);
+    };
+    // the backward tables of segment s: zero its window but the last column's, put the checkpoint there and sweep
+    auto resweep = [&](uint32_t s, GlSweep &sw, bool clear) {
+        const uint64_t base = beta_off(c[s]);
+        sw.beta_base = base;
+        sw.clear = clear ? beta_off(c[s + 1] - 1) - base : 0;
+        if (s + 1 < S) {
+            sw.copy_dst = beta_off(c[s + 1] - 1) - base;
+            sw.copy_src = ckpt[s];
+            sw.copy_n = own(c[s + 1] - 1);
+        }
+        sw.bwd_begin = (uint32_t)out.steps.size();
+        for (uint32_t k = c[s + 1] - 1; k > c[s]; --k) backward(k, beta_off(k - 1) - base);
+    };
+    for (uint32_t s = S; s-- > 0;) {  // pass A (the store starts zeroed)
+        GlSweep sw{};
+        resweep(s, sw, s + 1 < S);
+        if (s > 0) backward(c[s], ckpt[s - 1]);
+        sw.bwd_end = sw.fwd_begin = sw.fwd_end = (uint32_t)out.steps.size();
+        out.sweeps.push_back(sw);
+    }
+    for (uint32_t s = 0; s < S; ++s) {  // pass B
+        GlSweep sw{};
+        if (s > 0) resweep(s, sw, true);
+        else {
+            sw.beta_base = beta_off(c[0]);
+            sw.bwd_begin = (uint32_t)out.steps.size();
+        }
+        sw.bwd_end = sw.fwd_begin = (uint32_t)out.steps.size();
+        for (uint32_t k = c[s]; k < c[s + 1]; ++k) {  // as gl_schedule's forward steps of a one-table group
+            const uint32_t i = k - lo;
+            GlStep st{};
+            st.k = k;
+            st.cells_log2 = g.cols[k].a;
+            st.cur_off = (uint64_t)(i & 1) * f_size;
+            st.prev_off = (uint64_t)((i + 1) & 1) * f_size;
+            st.n_scale = own(k);
+            st.n_clear = f_size;
+            out.steps.push_back(st);
+        }
+        sw.fwd_end = (uint32_t)out.steps.size();
+        out.sweeps.push_back(sw);
+    }
     return true;
+}
+
+int gl_plan(const GlPacked &g, uint32_t T, uint64_t budget, std::vector<GlUnit> &units, std::string &err) {
+    std::vector<uint32_t> begin;
+    std::vector<uint8_t> alone;
+    gl_groups_split(g, T, budget, begin, alone);
+    units.assign(alone.size(), GlUnit());
+    uint64_t need = 0;  // > 0: the least budget that the refused tables fit
+    for (size_t q = 0; q < units.size(); ++q) {
+        GlUnit &u = units[q];
+        u.bounded = alone[q];
+        if (!u.bounded) {
+            gl_schedule(g, T, begin[q], begin[q + 1], u.sc);
+            u.work_doubles = u.sc.beta_doubles + 1 + u.sc.f_pool_doubles;
+        } else if (gl_bounded(g, T, begin[q], begin[q + 1], budget, u.bd)) {
+            u.work_doubles = u.bd.arena_doubles + u.bd.ckpt_doubles + u.bd.f_pool_doubles;
+        } else {  // the least budget with a cut that fits (bisection), at most the table's resident cost
+            GlSchedule whole;
+            gl_schedule(g, T, begin[q], begin[q + 1], whole);
+            uint64_t no = budget, yes = whole.beta_doubles + whole.f_pool_doubles;
+            GlBounded probe;
+            while (yes - no > 1) {
+                const uint64_t mid = no + (yes - no) / 2;
+                (gl_bounded(g, T, begin[q], begin[q + 1], mid, probe) ? yes : no) = mid;
+            }
+            need = std::max(need, yes);
+        }
+    }
+    if (need) {
+        err = "genotyping: " + std::to_string(budget * 8) + " bytes for backward tables and projection buffers hold no segment of a table; it needs at least " +
+              std::to_string(need * 8) + " bytes";
+        return WHMEC_ERR_UNSUPPORTED;
+    }
+    return WHMEC_OK;
 }
 
 void gl_scale_host(double *v, uint64_t n) {

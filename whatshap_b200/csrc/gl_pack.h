@@ -44,6 +44,46 @@ void gl_schedule(const GlPacked &g, uint32_t T, uint32_t lo, uint32_t hi, GlSche
 // `budget` doubles: group q = columns [begin[q], begin[q + 1]).  False if a single table exceeds the budget.
 bool gl_groups(const GlPacked &g, uint32_t T, uint64_t budget, std::vector<uint32_t> &begin);
 
+// The same groups, except that a table which alone exceeds the budget becomes a group of its own with alone[q] = 1
+// (alone[q] = 0 for the other groups).  Without such a table the groups are those of gl_groups.
+void gl_groups_split(const GlPacked &g, uint32_t T, uint64_t budget, std::vector<uint32_t> &begin, std::vector<uint8_t> &alone);
+
+// Memory-bounded forward-backward of one table, columns [lo, hi), whose backward tables do not fit (DESIGN §4.5).
+// Segment s = columns [cuts[s], cuts[s + 1]).  All segments share an arena at the start of the backward store; behind it
+// sit the checkpoints, one per segment but the last: the scaled backward table of the segment's last column.
+// Pass A runs the backward steps of the whole table right to left, segment by segment; the step of a segment's first
+// column writes into the checkpoint of the segment to its left.  Pass B runs left to right: every segment but the first
+// (whose backward tables pass A left in the arena) first sweeps its backward steps again from its checkpoint (the last
+// segment from B = 1), then runs its forward steps.  One launch per step; the projection buffers carry across segments.
+struct GlSweep {             // one segment's part of pass A or pass B, in this order:
+    uint64_t beta_base;      //   B_k of the segment's columns sits at store + cols[k].beta_off - beta_base
+    uint64_t clear;          //   zero store[0, clear) (the backward steps accumulate)
+    uint64_t copy_dst, copy_src, copy_n;  // copy store[copy_src, +copy_n) to store[copy_dst] (copy_n = 0: none)
+    uint32_t bwd_begin, bwd_end;          // backward steps [bwd_begin, bwd_end), then
+    uint32_t fwd_begin, fwd_end;          // forward steps [fwd_begin, fwd_end)
+};
+struct GlBounded {
+    std::vector<GlStep> steps;           // offsets: backward into the store, forward into the F pool
+    std::vector<GlSweep> sweeps;         // pass A, then pass B
+    std::vector<uint32_t> cuts;          // cuts[0] = lo, cuts.back() = hi
+    uint64_t arena_doubles = 0, ckpt_doubles = 0;  // the store: arena, then the checkpoints
+    uint64_t f_pool_doubles = 0;         // the table's two projection buffers
+};
+// Cuts with bounded.h's cut_column_segments applied to the mirrored column order, so that the first segment, the one
+// swept backward only once, is as large as fits.  The store + F pool stay within `budget` doubles; false when no cut fits.
+bool gl_bounded(const GlPacked &g, uint32_t T, uint32_t lo, uint32_t hi, uint64_t budget, GlBounded &out);
+
+// Everything one genotyping call runs under `budget` doubles for backward tables, checkpoints and projection buffers:
+// groups of whole tables (gl_groups_split; gl_schedule) and, for a table that alone exceeds the budget, its bounded plan.
+struct GlUnit {
+    bool bounded;
+    GlSchedule sc;         // !bounded
+    GlBounded bd;          // bounded
+    uint64_t work_doubles; // store + F pool: backward tables (+ 1 spare) or arena + checkpoints, and projection buffers
+};
+// WHMEC_ERR_UNSUPPORTED when a table has no cut that fits; `err` then states a budget that fits ("needs at least N bytes").
+int gl_plan(const GlPacked &g, uint32_t T, uint64_t budget, std::vector<GlUnit> &units, std::string &err);
+
 // Packs `p` (whose gl holds the genotype priors; gt and distrust are ignored) for the genotyping DP.
 int gl_pack(const whmec_problem *p, Packed &pk, GlPacked &g, std::string &err);
 
