@@ -1,4 +1,4 @@
-"""Resident vs memory-bounded pedigree sweeps on the GPU (DESIGN §4.3).
+"""Resident vs memory-bounded pedigree sweeps on the GPU (DESIGN §4.2).
 
   python scripts/ped_memory_bounded.py [--cfg5-cols 20000] [--reps 3] [--family-cols N] [--leave-free-gb G] [--out FILE]
 

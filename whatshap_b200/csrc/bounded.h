@@ -1,4 +1,4 @@
-// Segment cutter of the memory-bounded column / pedigree sweep (whmec.cu, DESIGN §4.3): when the back-pointers of the whole
+// Segment cutter of the memory-bounded column / pedigree sweep (col_plan.cpp, DESIGN §4.2): when the back-pointers of the whole
 // table exceed the budget, the table is cut into segments that share one arena.  Host only, so that the test harness
 // (tests/emul) checks the cuts on the CPU.
 //

@@ -29,6 +29,7 @@ constexpr uint32_t PF_INF = 1u << 30;   // +infinity of this path (UMAX at the b
 constexpr uint32_t PF_MAX_A = 16;       // active reads per column (two byte tables)
 constexpr uint32_t PF_MAX_F = 12;       // log2 projection entries per transmission value
 constexpr uint32_t PF_THREADS = 1024;
+constexpr uint32_t PF_MAX_CLUSTER = 8;  // CTAs per chain of ped_fused_cluster_kernel (whmec.cu), at most
 
 constexpr uint32_t PF_ROW = 20;         // words per row of a byte table: 16 slots + 4 words of skew (rows 0..7 start in 8 different
                                         // groups of four banks, so the 128-bit loads of a quarter warp spread over all banks)

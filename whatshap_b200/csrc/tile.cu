@@ -790,6 +790,7 @@ int TilePlan::create(const Packed &pk, cudaStream_t stream, uint64_t &h2d, std::
     const uint64_t resident_limit = arena_override ? std::min(arena_override, budget) : budget;
     if ((ts.bp_words + 1) * 4 <= resident_limit || n_rounds <= 1) {
         if ((ts.bp_words + 1) * 4 > resident_limit) {
+            over_hbm = true;
             msg = "tile path: state + back-pointer storage exceeds the free HBM of this device";
             return WHMEC_ERR_UNSUPPORTED;
         }
@@ -829,6 +830,7 @@ int TilePlan::create(const Packed &pk, cudaStream_t stream, uint64_t &h2d, std::
             }
         }
         if (!ok) {
+            over_hbm = true;
             msg = "tile path: state + back-pointer storage exceeds the free HBM of this device";
             return WHMEC_ERR_UNSUPPORTED;
         }

@@ -16,6 +16,7 @@ struct TilePlan {
     uint64_t state_bytes = 0;     // projection state moved through global memory by one sweep
     uint32_t launches = 0;
     std::string why;              // reason when plan() returns false
+    bool over_hbm = false;        // create() refused: state + back-pointers exceed the free HBM
     void *impl = nullptr;
     // Host-only: decide whether the tile path applies and build its schedule.
     bool plan(const Packed &pk);

@@ -24,7 +24,7 @@
 #include <vector>
 
 #include "../../include/whmec.h"
-#include "bounded.h"
+#include "col_plan.h"
 #include "common.h"
 #include "dp_device.h"
 #include "ped_fused.h"
@@ -154,15 +154,6 @@ __device__ __forceinline__ ColView make_view(const ColShared &S, uint32_t T, uin
     return v;
 }
 
-// lanes per projection entry (log2): one thread per entry when the column has enough entries to fill
-// the GPU, otherwise the 2^d candidates of an entry are spread over up to 32 lanes
-__host__ __device__ inline uint32_t col_lane_bits(uint32_t log_entries, uint32_t d) {
-    if (log_entries >= 14) return 0;
-    const uint32_t want = 14 - log_entries;
-    const uint32_t lc = d < want ? d : want;
-    return lc < 5 ? lc : 5;
-}
-
 // Body of the per-column kernels for d <= 7: thread (or lane group) per projection entry.
 __device__ __forceinline__ void direct_body(ColShared &S, uint32_t *bpvals, uint32_t T, uint32_t tb,
                                             const uint32_t *fn_c0, const int32_t *fn_delta, const uint32_t *prev,
@@ -241,16 +232,8 @@ __global__ void __launch_bounds__(256) col_direct_kernel(const __grid_constant__
 // input vector; pass 2 re-sweeps every chain with its true input, writing the same back-pointers
 // the sequential sweep would write (SURVEY.md section 8(e), verified there against the reference).
 // All chains advance together: one launch = one column step of every (chain, input) instance.
+// The step lists (PedStep) are planned by col_plan.cpp.
 // ------------------------------------------------------------------------------------------
-struct PedStep {
-    ColMeta cm;
-    uint32_t nf;
-    uint32_t slot;   // state slot of the instance (two value buffers per slot)
-    uint32_t flags;  // bit 0: write back-pointers; bit 1: write transition minima for the next column;
-                     // bit 2: the previous projection holds transition minima
-    uint32_t rc_next;
-};
-
 __global__ void __launch_bounds__(256) col_batched_kernel(const PedStep *__restrict__ steps, uint32_t *__restrict__ vals,
                                                           uint64_t max_ent, uint32_t T, uint32_t tb,
                                                           const uint32_t *__restrict__ fn_c0, const int32_t *__restrict__ fn_delta,
@@ -521,7 +504,6 @@ __global__ void __launch_bounds__(PF_THREADS, 1) ped_fused_kernel(const PedFused
 // cluster through distributed shared memory.  One cluster barrier per column orders those writes against the next column's
 // reads; columns with fewer than 32 outputs per CTA are computed by every CTA redundantly (no exchange).
 constexpr size_t PF_CLUSTER_SMEM = PF_COL_BYTES + (size_t)PF_MAX_ENT * 2 * (4 + 1);
-constexpr uint32_t PF_MAX_CLUSTER = 8;
 
 __global__ void __launch_bounds__(PF_THREADS, 1) ped_fused_cluster_kernel(const PedFusedArgs a) {
     namespace cg = cooperative_groups;
@@ -1153,16 +1135,12 @@ struct whmec_plan {
     DevBuf<int32_t> d_fn_delta;
     DevBuf<unsigned long long> d_keys;
     uint32_t last_buf = 0;
+    ColPlan col;  // which column-kernel sweep, its memory-bounded segments and batched step lists (col_plan.h)
     // batched pedigree sweep (see col_batched_kernel)
-    bool use_ped_batch = false;
     DevBuf<PedStep> d_ped_steps;
     DevBuf<uint32_t> d_ped_vals, d_chain_len;
     DevBuf<uint8_t> d_ped_args;
-    std::vector<uint32_t> ped_begin[3], ped_grid[3];  // [0] pass 1 (per-input instances), [1] pass 2, [2] pass 1 multi-RHS
-    bool ped_multi = false;
-    uint64_t ped_max_ent = 0;
-    uint32_t ped_slots = 0;
-    const uint32_t *d_last_vals = nullptr;
+    const uint32_t *d_last_vals = nullptr;  // two-pass sweeps: the last chain's final values
     // segment of a pedigree table shared by several GPUs (whmec_segment_*): 0 = whole table,
     // 1 = first segment, 2 = segment continuing a table (its first column receives an input vector)
     int segment = 0;
@@ -1170,18 +1148,10 @@ struct whmec_plan {
     int exits_mode = 0;  // 0: not computed since the last sweep; 1: last chain entered at the optimum; 2: like any chain
     DevBuf<uint32_t> d_in_vec, d_matrix, d_bt_exits, d_bt_entries;
     // fused trio sweep (ped_fused_kernel / ped_fused_cluster_kernel, ped_fused.h)
-    bool use_ped_fused = false;
-    uint32_t ped_cluster = 1;  // CTAs per chain of the fused pedigree sweep
     DevBuf<uint32_t> d_chain_rows, d_chain_in, d_chain_out;
     uint32_t sweeps_done = 0;
     cudaGraphExec_t graph_exec = nullptr;
-    // memory-bounded sweep (back-pointers beyond the budget, DESIGN §4.3): segments share one arena (ColMeta::bp_off rebased to the
-    // segment's first column); the sweep leaves the last segment's back-pointers there, the backtrace sweeps the others right to left
-    bool bounded = false;
-    std::vector<uint32_t> seg_col;    // sequential path: column cuts, segment s = columns [seg_col[s], seg_col[s + 1])
-    std::vector<uint64_t> seg_ckpt;   // sequential path: word offset in d_ckpt of the values column seg_col[s] - 1 hands on (s >= 1)
-    std::vector<uint32_t> seg_chain;  // two-pass paths: chain cuts, segment s = chains [seg_chain[s], seg_chain[s + 1])
-    std::vector<std::vector<uint32_t>> seg_begin, seg_grid;  // batched path: pass-2 steps of every segment (as ped_begin / ped_grid)
+    // memory-bounded sweep (DESIGN §4.2): the backtrace sweeps the segments of col right to left
     uint32_t arena_seg = 0;           // segment whose back-pointers are in the arena
     DevBuf<uint32_t> d_ckpt, d_bt_state;
     // tile path
@@ -1219,6 +1189,80 @@ void keep_host_memory() {
     if (e && e[0] == '0') return;
     mallopt(M_MMAP_THRESHOLD, 1 << 30);
     mallopt(M_TRIM_THRESHOLD, 1 << 30);
+}
+
+// Column-kernel paths: plans with col_plan, then allocates and uploads what the plan lists (on the plan's stream).
+int col_create(whmec_plan *pl, bool bounded_t1, uint64_t &h2d, std::string &msg) {
+    Packed &pk = pl->pk;
+    const uint32_t n = pk.n;
+    // what col_plan decides from: the free device memory, the multiprocessors and the column path's switches (DESIGN §10)
+    ColPlanInput in;
+    in.free_bytes = device_available_bytes();
+    if (const char *e = std::getenv("WHMEC_COLUMN_ARENA_BUDGET")) in.hook = std::max<uint64_t>(8, std::strtoull(e, nullptr, 10));
+    const char *pf = std::getenv("WHMEC_PED_FUSED"), *seq = std::getenv("WHMEC_PED_SEQUENTIAL"), *cl = std::getenv("WHMEC_PED_CLUSTER");
+    in.fused = !(pf && pf[0] == '0');
+    in.sequential = seq && seq[0] == '1';
+    in.cluster = cl ? (uint32_t)std::atoi(cl) : 0;
+    in.segment = pl->segment;
+    in.bounded_t1 = bounded_t1;
+    int sms = 132;
+    CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, pl->device));
+    in.sms = (uint32_t)sms;
+    const int rc = col_plan(pk, in, pl->col, msg);
+    if (rc != WHMEC_OK) return rc;
+    const ColPlan &cp = pl->col;
+    const uint32_t C = (uint32_t)pk.chain_begin.size() - 1;
+    if (cp.bounded) pl->stats.backptr_bytes = cp.arena_words * 4;
+    if (!pl->d_cols.p) CUDA_TRY(pl->d_cols.alloc(n, pl->stream));  // (already there when the tile planner declined the problem)
+    CUDA_TRY(pl->d_fn_c0.alloc(pk.fn_c0.size(), pl->stream));
+    CUDA_TRY(pl->d_fn_delta.alloc(pk.fn_delta.size(), pl->stream));
+    CUDA_TRY(pl->d_fn_group.alloc(pk.fn_group.size(), pl->stream));
+    CUDA_TRY(pl->d_chain_begin.alloc(pk.chain_begin.size(), pl->stream));
+    CUDA_TRY(pl->d_val[0].alloc(cp.max_ent, pl->stream));
+    CUDA_TRY(pl->d_val[1].alloc(cp.max_ent, pl->stream));
+    CUDA_TRY(pl->d_keys.alloc(cp.max_ent, pl->stream));
+    CUDA_TRY(pl->d_arena.alloc(cp.arena_words + 1, pl->stream));
+    if (cp.bounded) {
+        CUDA_TRY(pl->d_ckpt.alloc(cp.ckpt_words, pl->stream));
+        CUDA_TRY(pl->d_bt_state.alloc(2, pl->stream));
+        pl->arena_seg = (uint32_t)(cp.seg_chain.empty() ? cp.seg_col.size() : cp.seg_chain.size()) - 2;
+    }
+    auto up = [&](void *dst, const void *src, size_t bytes) {
+        h2d += bytes;
+        return cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, pl->stream);
+    };
+    CUDA_TRY(up(pl->d_cols.p, pk.cols.data(), (size_t)n * sizeof(ColMeta)));
+    CUDA_TRY(up(pl->d_fn_c0.p, pk.fn_c0.data(), pk.fn_c0.size() * 4));
+    CUDA_TRY(up(pl->d_fn_delta.p, pk.fn_delta.data(), pk.fn_delta.size() * 4));
+    CUDA_TRY(up(pl->d_fn_group.p, pk.fn_group.data(), pk.fn_group.size() * 4));
+    CUDA_TRY(up(pl->d_chain_begin.p, pk.chain_begin.data(), pk.chain_begin.size() * 4));
+    pl->stats.path_kind = cp.path == ColPath::column ? 2 : 3;
+    if (cp.path == ColPath::fused) {
+        CUDA_TRY(pl->d_chain_rows.alloc((size_t)C * PF_T, pl->stream));
+        CUDA_TRY(pl->d_chain_in.alloc((size_t)C * PF_T, pl->stream));
+        CUDA_TRY(pl->d_chain_out.alloc((size_t)C * PF_T, pl->stream));
+        CUDA_TRY(cudaFuncSetAttribute(ped_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PF_SMEM));
+        CUDA_TRY(cudaFuncSetAttribute(ped_fused_cluster_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PF_CLUSTER_SMEM));
+        pl->d_last_vals = pl->d_chain_out.p + (size_t)(C - 1) * PF_T;
+    } else if (cp.path == ColPath::batched) {
+        CUDA_TRY(pl->d_ped_steps.alloc(cp.steps.size(), pl->stream));
+        CUDA_TRY(pl->d_ped_vals.alloc(cp.slots * 2 * cp.max_ent, pl->stream));
+        CUDA_TRY(pl->d_ped_args.alloc(cp.slots * 2 * cp.max_ent, pl->stream));
+        CUDA_TRY(pl->d_chain_len.alloc(C, pl->stream));
+        CUDA_TRY(up(pl->d_ped_steps.p, cp.steps.data(), cp.steps.size() * sizeof(PedStep)));
+        CUDA_TRY(up(pl->d_chain_len.p, cp.clen.data(), C * 4));
+        const uint32_t last_slot = C * pk.T + (C - 1);
+        pl->d_last_vals = pl->d_ped_vals.p + ((uint64_t)last_slot * 2 + ((cp.clen[C - 1] - 1) & 1u)) * cp.max_ent;
+    }
+    if (pk.T > 1) {
+        CUDA_TRY(pl->d_bt_exits.alloc((size_t)C * pk.T, pl->stream));
+        CUDA_TRY(pl->d_bt_entries.alloc(C, pl->stream));
+    }
+    if (pl->segment) {
+        CUDA_TRY(pl->d_in_vec.alloc(pk.T, pl->stream));
+        CUDA_TRY(pl->d_matrix.alloc((size_t)pk.T * pk.T, pl->stream));
+    }
+    return WHMEC_OK;
 }
 
 // bounded_t1: a single individual whose back-pointers exceed the free HBM takes the memory-bounded sweep (solve_impl, once no
@@ -1273,7 +1317,6 @@ int plan_create_impl(const whmec_problem *p, int device, whmec_plan *pl, std::st
         rc = pack_problem(p, pl->pk, msg, true);
         if (rc != WHMEC_OK) return rc;
     }
-    pl->device = device;
     pl->stats = pk.stats;
     if (segment) {
         if (pk.T == 1 || pk.n == 0) {
@@ -1307,235 +1350,8 @@ int plan_create_impl(const whmec_problem *p, int device, whmec_plan *pl, std::st
         pl->stats.path_kind = 1;
         pl->stats.backptr_bytes = pl->tiles.backptr_bytes;
     } else {
-        const size_t free_b = device_available_bytes();
-        uint64_t max_ent = 1;
-        for (const ColMeta &m : pk.cols) max_ent = std::max<uint64_t>(max_ent, ((uint64_t)1 << m.f) * pk.T);
-        uint64_t need = pk.bp_words * 4 + max_ent * (4 * 2 + 8) + pk.fn_delta.size() * 4 + (uint64_t)n * sizeof(ColMeta);
-        constexpr uint64_t RESERVE = 512ull << 20;
-        const uint64_t fixed = need - pk.bp_words * 4;  // everything but the back-pointers
-        const uint64_t hbm_budget = free_b > fixed + RESERVE ? free_b - fixed - RESERVE : 0;
-        // WHMEC_COLUMN_ARENA_BUDGET=bytes (test hook): back-pointers beyond it take the memory-bounded sweep; the budget is the arena's,
-        // checkpoints come on top (as with WHMEC_TILE_ARENA_BUDGET).  Without it the budget is the free HBM and covers both.
-        uint64_t hook = 0;
-        if (const char *e = std::getenv("WHMEC_COLUMN_ARENA_BUDGET")) hook = std::max<uint64_t>(8, std::strtoull(e, nullptr, 10));
-        const bool over_hbm = need + RESERVE > free_b, over_hook = hook && pk.bp_words * 4 > hook;
-        // single individuals: solve_impl first solves groups of chains one after another (grouped.h); the bounded sweep is for
-        // what no group size fits (bounded_t1)
-        const bool bounded = !segment && (over_hook || (over_hbm && (pk.T > 1 || bounded_t1)));
-        if (over_hbm && !bounded) {
-            msg = "back-pointer storage exceeds the free HBM of this device";
-            return WHMEC_ERR_UNSUPPORTED;
-        }
-        // which sweep: pedigrees with several chains take a two-pass sweep (fused trio kernel or batched), the rest the column sweep
-        const char *seq = std::getenv("WHMEC_PED_SEQUENTIAL");
-        const uint32_t C = (uint32_t)pk.chain_begin.size() - 1;
-        // one trio, shapes of ped_fused.h: one block per chain with the projection in shared memory (3 launches)
-        bool fused_ok = false;
-        {
-            const char *pf = std::getenv("WHMEC_PED_FUSED");
-            fused_ok = !(pf && pf[0] == '0') && pk.T == PF_T && (C >= 2 || segment) && pk.safe31 && !(seq && seq[0] == '1' && !segment);
-            for (uint32_t k = 0; k < n && fused_ok; ++k) fused_ok = pf_column_ok(pk.cols[k], pk.fn_group.data() + pk.cols[k].grp_off);
-        }
-        // batched sweep: the batch buffers (values + argmins of every (chain, unit vector) instance) count against the free HBM as well
-        const uint64_t slots = (uint64_t)C * pk.T + C, batch_bytes = slots * 2 * max_ent * 5;
-        auto batch_ok = [&](uint64_t arena_bytes) {
-            return pk.T > 1 && (C >= 2 || segment) && pk.safe31 && !(seq && seq[0] == '1' && !segment) && slots * 2 * max_ent * 4 < (8ull << 30) &&
-                   (uint64_t)C * pk.T <= 65535 && fixed + arena_bytes + batch_bytes + RESERVE <= free_b;
-        };
-        uint64_t arena_words = pk.bp_words, ckpt_words = 0;
-        bool two_pass = true;  // (resident: whatever the conditions above allow)
-        if (bounded) {
-            std::vector<uint64_t> off(n + 1);
-            for (uint32_t k = 0; k < n; ++k) off[k] = pk.cols[k].bp_off;
-            off[n] = pk.bp_words;
-            // two-pass paths: segments of whole chains, after pass 1 every chain's input is known (no checkpoints)
-            two_pass = false;
-            if (fused_ok || batch_ok(0)) {
-                const uint64_t b2 = over_hook ? hook : fused_ok ? hbm_budget : (hbm_budget > batch_bytes ? hbm_budget - batch_bytes : 0);
-                two_pass = cut_chain_segments(pk.chain_begin, off, b2 / 4, pl->seg_chain, arena_words) && (fused_ok || batch_ok(arena_words * 4));
-            }
-            if (two_pass) {
-                for (size_t sg = 0; sg + 1 < pl->seg_chain.size(); ++sg) {
-                    const uint32_t k0 = pk.chain_begin[pl->seg_chain[sg]], k1 = pk.chain_begin[pl->seg_chain[sg + 1]];
-                    for (uint32_t k = k0; k < k1; ++k) pk.cols[k].bp_off -= off[k0];
-                }
-            } else {  // a chain alone exceeds the budget, or no two-pass sweep: column sweep with checkpoints
-                pl->seg_chain.clear();
-                fused_ok = false;
-                std::vector<uint64_t> ck(n);
-                uint64_t widest = 0, widest_ck = 0;
-                for (uint32_t k = 0; k < n; ++k) {
-                    ck[k] = ((uint64_t)1 << pk.cols[k].f) * pk.T;
-                    widest = std::max(widest, off[k + 1] - off[k]);
-                    widest_ck = std::max(widest_ck, ck[k]);
-                }
-                const bool fits = over_hook ? cut_column_segments(off, {}, hook / 4, pl->seg_col, arena_words, ckpt_words) &&
-                                                  fixed + 4 * (arena_words + ckpt_words) + RESERVE <= free_b
-                                            : cut_column_segments(off, ck, hbm_budget / 4, pl->seg_col, arena_words, ckpt_words);
-                if (!fits) {
-                    msg = over_hook ? "memory-bounded sweep: an arena of " + std::to_string(hook) + " bytes holds no segment; it needs at least " +
-                                          std::to_string(4 * widest) + " bytes (the widest column's back-pointers), checkpoints on top"
-                                    : "memory-bounded sweep: " + std::to_string(hbm_budget) + " bytes of free HBM hold no segment; it needs at least " +
-                                          std::to_string(4 * (widest + widest_ck)) + " bytes (the widest column's back-pointers and the largest checkpoint)";
-                    return WHMEC_ERR_UNSUPPORTED;
-                }
-                if (over_hook)
-                    for (size_t sg = 1; sg + 1 < pl->seg_col.size(); ++sg) ckpt_words += ck[pl->seg_col[sg] - 1];
-                pl->seg_ckpt.assign(pl->seg_col.size() - 1, 0);
-                uint64_t at = 0;
-                for (size_t sg = 0; sg + 1 < pl->seg_col.size(); ++sg) {
-                    const uint32_t k0 = pl->seg_col[sg], k1 = pl->seg_col[sg + 1];
-                    for (uint32_t k = k0; k < k1; ++k) pk.cols[k].bp_off -= off[k0];
-                    if (sg) {
-                        pl->seg_ckpt[sg] = at;
-                        at += ck[k0 - 1];
-                    }
-                }
-            }
-            pl->bounded = true;
-            pl->stats.backptr_bytes = arena_words * 4;
-        }
-        if (!pl->d_cols.p) CUDA_TRY(pl->d_cols.alloc(n, pl->stream));  // (already there when the tile planner declined the problem)
-        CUDA_TRY(pl->d_fn_c0.alloc(pk.fn_c0.size(), pl->stream));
-        CUDA_TRY(pl->d_fn_delta.alloc(pk.fn_delta.size(), pl->stream));
-        CUDA_TRY(pl->d_fn_group.alloc(pk.fn_group.size(), pl->stream));
-        CUDA_TRY(pl->d_chain_begin.alloc(pk.chain_begin.size(), pl->stream));
-        CUDA_TRY(pl->d_val[0].alloc(max_ent, pl->stream));
-        CUDA_TRY(pl->d_val[1].alloc(max_ent, pl->stream));
-        CUDA_TRY(pl->d_keys.alloc(max_ent, pl->stream));
-        CUDA_TRY(pl->d_arena.alloc(arena_words + 1, pl->stream));
-        if (pl->bounded) {
-            CUDA_TRY(pl->d_ckpt.alloc(ckpt_words, pl->stream));
-            CUDA_TRY(pl->d_bt_state.alloc(2, pl->stream));
-            pl->arena_seg = (uint32_t)(two_pass ? pl->seg_chain.size() : pl->seg_col.size()) - 2;
-        }
-        auto up = [&](void *dst, const void *src, size_t bytes) {
-            h2d += bytes;
-            return cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, pl->stream);
-        };
-        CUDA_TRY(up(pl->d_cols.p, pk.cols.data(), (size_t)n * sizeof(ColMeta)));
-        CUDA_TRY(up(pl->d_fn_c0.p, pk.fn_c0.data(), pk.fn_c0.size() * 4));
-        CUDA_TRY(up(pl->d_fn_delta.p, pk.fn_delta.data(), pk.fn_delta.size() * 4));
-        CUDA_TRY(up(pl->d_fn_group.p, pk.fn_group.data(), pk.fn_group.size() * 4));
-        CUDA_TRY(up(pl->d_chain_begin.p, pk.chain_begin.data(), pk.chain_begin.size() * 4));
-        pl->stats.path_kind = 2;
-        if (fused_ok) {
-            CUDA_TRY(pl->d_chain_rows.alloc((size_t)C * PF_T, pl->stream));
-            CUDA_TRY(pl->d_chain_in.alloc((size_t)C * PF_T, pl->stream));
-            CUDA_TRY(pl->d_chain_out.alloc((size_t)C * PF_T, pl->stream));
-            CUDA_TRY(cudaFuncSetAttribute(ped_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PF_SMEM));
-            CUDA_TRY(cudaFuncSetAttribute(ped_fused_cluster_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PF_CLUSTER_SMEM));
-            {   // fewer chains than SMs: a cluster of 2 / 4 / 8 CTAs per chain (WHMEC_PED_CLUSTER=n forces n, 1 = off)
-                int dev = 0, sms = 132;
-                CUDA_TRY(cudaGetDevice(&dev));
-                CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-                uint32_t cs = 1;
-                while (cs * 2 <= PF_MAX_CLUSTER && (uint64_t)C * cs * 2 <= (uint64_t)sms) cs *= 2;
-                if (const char *e = std::getenv("WHMEC_PED_CLUSTER")) {
-                    const int want = std::atoi(e);
-                    if (want == 1 || want == 2 || want == 4 || want == 8) cs = (uint32_t)want;
-                }
-                pl->ped_cluster = cs;
-            }
-            pl->use_ped_fused = true;
-            pl->use_ped_batch = true;  // two-pass sweep: the backtrace and the optimum read the chains' final values
-            pl->d_last_vals = pl->d_chain_out.p + (size_t)(C - 1) * PF_T;
-            pl->stats.path_kind = 3;
-        } else if (two_pass && batch_ok(arena_words * 4)) {
-            const uint32_t T = pk.T;
-            {
-                std::vector<PedStep> steps;
-                std::vector<uint32_t> clen(C);
-                for (uint32_t c = 0; c < C; ++c) clen[c] = pk.chain_begin[c + 1] - pk.chain_begin[c];
-                auto blocks_for = [&](const ColMeta &m) -> uint32_t {
-                    const uint64_t nent = ((uint64_t)1 << m.f) * T;
-                    if (m.d > 7) return (uint32_t)nent;
-                    const uint64_t epb = 256u >> col_lane_bits(m.f + pk.tb, m.d);
-                    return (uint32_t)((nent + epb - 1) / epb);
-                };
-                pl->ped_multi = T <= MULTI_MAX;
-                // the steps of one pass over chains [c_lo, c_hi) (pass 1 of the memory-bounded sweep: one segment)
-                auto add_steps = [&](int pass, uint32_t c_lo, uint32_t c_hi, std::vector<uint32_t> &begin, std::vector<uint32_t> &grid) {
-                    uint32_t len = 0;
-                    for (uint32_t c = c_lo; c < c_hi; ++c) len = std::max(len, clen[c]);
-                    for (uint32_t st = 0; st < len; ++st) {
-                        begin.push_back((uint32_t)steps.size());
-                        uint32_t gmax = 0;
-                        // pass 0: chain 0 (true input) and, without the multi-RHS kernel, every (chain, unit vector);
-                        // pass 1: chains >= 1 with their true inputs; pass 2: one multi-RHS instance per chain >= 1
-                        // with the multi-RHS kernel pass 0 is empty: chain 0 (whose input is known: the first column
-                        // of the table ignores it) runs in pass 1 like every other chain
-                        const uint32_t c_begin = (pass == 0 && !pl->ped_multi) ? c_lo : (pass == 0 ? c_hi : c_lo);
-                        const uint32_t c_end = c_hi;
-                        for (uint32_t c = c_begin; c < c_end; ++c) {
-                            if (clen[c] <= st) continue;
-                            const uint32_t kcol = pk.chain_begin[c] + st;
-                            const ColMeta &m = pk.cols[kcol];
-                            const uint32_t reps = pass == 0 ? T : 1;
-                            // a column hands transition minima to the next one of its chain when the T values of a
-                            // projection index are produced inside one thread block
-                            auto xform = [&](uint32_t k) {
-                                const ColMeta &q = pk.cols[k];
-                                return k + 1 < pk.chain_begin[c + 1] && q.d <= 7 && T <= (256u >> col_lane_bits(q.f + pk.tb, q.d));
-                            };
-                            for (uint32_t u = 0; u < reps; ++u) {
-                                PedStep ps;
-                                ps.cm = m;
-                                ps.nf = pk.fn_group[m.grp_off + T];
-                                ps.slot = pass == 1 ? (C * T + c) : (c * T + u);
-                                ps.flags = pass == 1 ? 1u : 0u;
-                                if (xform(kcol)) ps.flags |= 2u;
-                                if (st > 0 && xform(kcol - 1)) ps.flags |= 4u;
-                                if (pass == 2 && st == 0) ps.flags |= 8u;
-                                ps.rc_next = kcol + 1 < pk.n ? pk.cols[kcol + 1].rc : 0;
-                                steps.push_back(ps);
-                            }
-                            gmax = std::max(gmax, blocks_for(m));
-                        }
-                        grid.push_back(gmax);
-                    }
-                    begin.push_back((uint32_t)steps.size());
-                };
-                for (int pass = 0; pass < 3; ++pass) {
-                    pl->ped_begin[pass].clear();
-                    pl->ped_grid[pass].clear();
-                    if (pass == 2 && !pl->ped_multi) continue;
-                    if (pass == 1 && pl->bounded) continue;  // per segment, below
-                    add_steps(pass, 0, C, pl->ped_begin[pass], pl->ped_grid[pass]);
-                }
-                if (pl->bounded) {
-                    const size_t S = pl->seg_chain.size() - 1;
-                    pl->seg_begin.assign(S, {});
-                    pl->seg_grid.assign(S, {});
-                    for (size_t sg = 0; sg < S; ++sg) add_steps(1, pl->seg_chain[sg], pl->seg_chain[sg + 1], pl->seg_begin[sg], pl->seg_grid[sg]);
-                }
-                CUDA_TRY(pl->d_ped_steps.alloc(steps.size(), pl->stream));
-                CUDA_TRY(pl->d_ped_vals.alloc((uint64_t)slots * 2 * max_ent, pl->stream));
-                CUDA_TRY(pl->d_ped_args.alloc((uint64_t)slots * 2 * max_ent, pl->stream));
-                CUDA_TRY(pl->d_chain_len.alloc(C, pl->stream));
-                CUDA_TRY(up(pl->d_ped_steps.p, steps.data(), steps.size() * sizeof(PedStep)));
-                CUDA_TRY(up(pl->d_chain_len.p, clen.data(), C * 4));
-                CUDA_TRY(cudaStreamSynchronize(pl->stream));  // `steps` and `clen` are stack-local
-                pl->ped_max_ent = max_ent;
-                pl->ped_slots = (uint32_t)slots;
-                pl->use_ped_batch = true;
-                const uint32_t last_slot = C * T + (C - 1);
-                pl->d_last_vals = pl->d_ped_vals.p + ((uint64_t)last_slot * 2 + ((clen[C - 1] - 1) & 1u)) * max_ent;
-                pl->stats.path_kind = 3;
-            }
-        }
-        if (segment && !pl->use_ped_batch) {
-            msg = "unsupported: this segment cannot run the two-pass pedigree sweep (costs beyond 2^28 or state beyond the budget)";
-            return WHMEC_ERR_UNSUPPORTED;
-        }
-        if (pk.T > 1) {
-            CUDA_TRY(pl->d_bt_exits.alloc((size_t)C * pk.T, pl->stream));
-            CUDA_TRY(pl->d_bt_entries.alloc(C, pl->stream));
-        }
-        if (segment) {
-            CUDA_TRY(pl->d_in_vec.alloc(pk.T, pl->stream));
-            CUDA_TRY(pl->d_matrix.alloc((size_t)pk.T * pk.T, pl->stream));
-        }
+        rc = col_create(pl, bounded_t1, h2d, msg);
+        if (rc != WHMEC_OK) return rc;
     }
     // No synchronisation here: the uploads (asynchronous DMA from the page-locked arrays of `pk` / the tile schedule, which live
     // as long as the plan) overlap whatever the host does next; the sweep's first launch queues behind them on the same stream.
@@ -1562,26 +1378,26 @@ int ped_pass(whmec_plan *pl, int pass, uint32_t &launches, std::string &msg, int
     const uint32_t T = pk.T, tb = pk.tb;
     if (pass == 0) {
         const uint32_t unit_slots = ((uint32_t)pk.chain_begin.size() - 1) * T;
-        ped_init_kernel<<<(unit_slots * T + 255) / 256, 256, 0, pl->stream>>>(pl->d_ped_vals.p, pl->ped_max_ent, T, unit_slots);
+        ped_init_kernel<<<(unit_slots * T + 255) / 256, 256, 0, pl->stream>>>(pl->d_ped_vals.p, pl->col.max_ent, T, unit_slots);
         ++launches;
     }
-    const std::vector<uint32_t> &begin = seg >= 0 ? pl->seg_begin[seg] : pl->ped_begin[pass];
-    const std::vector<uint32_t> &grids = seg >= 0 ? pl->seg_grid[seg] : pl->ped_grid[pass];
+    const std::vector<uint32_t> &begin = seg >= 0 ? pl->col.seg_begin[seg] : pl->col.ped_begin[pass];
+    const std::vector<uint32_t> &grids = seg >= 0 ? pl->col.seg_grid[seg] : pl->col.ped_grid[pass];
     const size_t nsteps = grids.size();
     for (size_t st = 0; st < nsteps; ++st) {
         const uint32_t b0 = begin[st], b1 = begin[st + 1];
         if (b1 > b0) {
             dim3 grid(grids[st], b1 - b0);
-            col_batched_kernel<<<grid, 256, 0, pl->stream>>>(pl->d_ped_steps.p + b0, pl->d_ped_vals.p, pl->ped_max_ent, T, tb,
+            col_batched_kernel<<<grid, 256, 0, pl->stream>>>(pl->d_ped_steps.p + b0, pl->d_ped_vals.p, pl->col.max_ent, T, tb,
                                                                pl->d_fn_c0.p, pl->d_fn_delta.p, pl->d_fn_group.p, pl->d_arena.p,
                                                                (uint32_t)(st & 1), pl->d_ped_args.p);
             ++launches;
         }
-        if (pass == 0 && pl->ped_multi && st < pl->ped_grid[2].size()) {
-            const uint32_t m0 = pl->ped_begin[2][st], m1 = pl->ped_begin[2][st + 1];
+        if (pass == 0 && pl->col.ped_multi && st < pl->col.ped_grid[2].size()) {
+            const uint32_t m0 = pl->col.ped_begin[2][st], m1 = pl->col.ped_begin[2][st + 1];
             if (m1 > m0) {
-                dim3 grid(pl->ped_grid[2][st], m1 - m0);
-                col_multi_kernel<<<grid, 256, 0, pl->stream>>>(pl->d_ped_steps.p + m0, pl->d_ped_vals.p, pl->ped_max_ent, T, tb,
+                dim3 grid(pl->col.ped_grid[2][st], m1 - m0);
+                col_multi_kernel<<<grid, 256, 0, pl->stream>>>(pl->d_ped_steps.p + m0, pl->d_ped_vals.p, pl->col.max_ent, T, tb,
                                                                  pl->d_fn_c0.p, pl->d_fn_delta.p, pl->d_fn_group.p, (uint32_t)(st & 1));
                 ++launches;
             }
@@ -1594,7 +1410,7 @@ int ped_pass(whmec_plan *pl, int pass, uint32_t &launches, std::string &msg, int
 // every chain's true input vector from the transfer matrices (in_vec: see ped_prefix_kernel)
 int ped_prefix(whmec_plan *pl, const uint32_t *d_in_vec, uint32_t &launches, std::string &msg) {
     const uint32_t C = (uint32_t)pl->pk.chain_begin.size() - 1;
-    ped_prefix_kernel<<<1, 32, 0, pl->stream>>>(pl->d_ped_vals.p, pl->ped_max_ent, pl->pk.T, C, pl->d_chain_len.p, d_in_vec,
+    ped_prefix_kernel<<<1, 32, 0, pl->stream>>>(pl->d_ped_vals.p, pl->col.max_ent, pl->pk.T, C, pl->d_chain_len.p, d_in_vec,
                                                  pl->segment == 2, nullptr);
     ++launches;
     CUDA_TRY(cudaGetLastError());
@@ -1610,15 +1426,15 @@ PedFusedArgs ped_fused_args(whmec_plan *pl, bool unit, uint32_t chain0) {
 // chains [c0, c0 + count); count == 0: all chains
 int ped_fused_pass(whmec_plan *pl, bool unit, std::string &msg, uint32_t c0 = 0, uint32_t count = 0) {
     const uint32_t C = count ? count : (uint32_t)pl->pk.chain_begin.size() - 1;
-    if (pl->ped_cluster > 1) {
+    if (pl->col.cluster > 1) {
         cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3(C * pl->ped_cluster);
+        cfg.gridDim = dim3(C * pl->col.cluster);
         cfg.blockDim = dim3(PF_THREADS);
         cfg.dynamicSmemBytes = PF_CLUSTER_SMEM;
         cfg.stream = pl->stream;
         cudaLaunchAttribute attr[1];
         attr[0].id = cudaLaunchAttributeClusterDimension;
-        attr[0].val.clusterDim.x = pl->ped_cluster;
+        attr[0].val.clusterDim.x = pl->col.cluster;
         attr[0].val.clusterDim.y = 1;
         attr[0].val.clusterDim.z = 1;
         cfg.attrs = attr;
@@ -1641,8 +1457,8 @@ int ped_fused_prefix(whmec_plan *pl, const uint32_t *d_in_vec, uint32_t *d_matri
 // pass 2 of the two-pass sweeps for the chains of segment `seg` of the memory-bounded sweep (their back-pointers -> the arena)
 int ped_segment_pass(whmec_plan *pl, uint32_t seg, uint32_t &launches, std::string &msg) {
     int rc;
-    if (pl->use_ped_fused) {
-        rc = ped_fused_pass(pl, false, msg, pl->seg_chain[seg], pl->seg_chain[seg + 1] - pl->seg_chain[seg]);
+    if (pl->col.path == ColPath::fused) {
+        rc = ped_fused_pass(pl, false, msg, pl->col.seg_chain[seg], pl->col.seg_chain[seg + 1] - pl->col.seg_chain[seg]);
         ++launches;
     } else {
         rc = ped_pass(pl, 1, launches, msg, (int)seg);
@@ -1651,31 +1467,30 @@ int ped_segment_pass(whmec_plan *pl, uint32_t seg, uint32_t &launches, std::stri
     return rc;
 }
 
-// three launches for the whole table (memory-bounded: pass 2 for the last segment only, the backtrace sweeps the others)
-int ped_fused_sweep(whmec_plan *pl, std::string &msg) {
-    int rc = ped_fused_pass(pl, true, msg);
-    if (rc == WHMEC_OK) rc = ped_fused_prefix(pl, nullptr, nullptr, msg);
-    uint32_t launches = 2;
-    if (rc == WHMEC_OK) {
-        if (pl->bounded) {
-            rc = ped_segment_pass(pl, (uint32_t)pl->seg_chain.size() - 2, launches, msg);
-        } else {
-            rc = ped_fused_pass(pl, false, msg);
-            ++launches;
-        }
+// The two-pass sweep: pass 1 (unit inputs, values only), prefix, pass 2 (true inputs, back-pointers); one launch each on the fused
+// path.  Memory-bounded: pass 2 for the last segment only, the backtrace sweeps the others.
+int ped_two_pass_sweep(whmec_plan *pl, std::string &msg) {
+    const bool fused = pl->col.path == ColPath::fused;
+    uint32_t launches = fused ? 2 : 0;
+    int rc = fused ? ped_fused_pass(pl, true, msg) : ped_pass(pl, 0, launches, msg);
+    if (rc == WHMEC_OK) rc = fused ? ped_fused_prefix(pl, nullptr, nullptr, msg) : ped_prefix(pl, nullptr, launches, msg);
+    if (rc == WHMEC_OK && pl->col.bounded) {
+        rc = ped_segment_pass(pl, (uint32_t)pl->col.seg_chain.size() - 2, launches, msg);
+    } else if (rc == WHMEC_OK && fused) {
+        rc = ped_fused_pass(pl, false, msg);
+        ++launches;
+    } else if (rc == WHMEC_OK) {
+        rc = ped_pass(pl, 1, launches, msg);
     }
     pl->stats.kernel_launches = launches;
     return rc;
 }
 
-int ped_batched_sweep(whmec_plan *pl, std::string &msg) {
-    if (pl->use_ped_fused) return ped_fused_sweep(pl, msg);
-    uint32_t launches = 0;
-    int rc = ped_pass(pl, 0, launches, msg);
-    if (rc == WHMEC_OK) rc = ped_prefix(pl, nullptr, launches, msg);
-    if (rc == WHMEC_OK) rc = pl->bounded ? ped_segment_pass(pl, (uint32_t)pl->seg_chain.size() - 2, launches, msg) : ped_pass(pl, 1, launches, msg);
-    pl->stats.kernel_launches = launches;
-    return rc;
+// an enqueue failed while the stream was being captured into a graph: do not leave the stream in capture mode
+void end_capture(whmec_plan *pl) {
+    cudaGraph_t dead = nullptr;
+    cudaStreamEndCapture(pl->stream, &dead);
+    if (dead) cudaGraphDestroy(dead);
 }
 
 // Column k of the column sweep: reads the values of column k - 1 from `prev`, writes its own to `out` and its back-pointers to the
@@ -1695,11 +1510,7 @@ int column_launch(whmec_plan *pl, uint32_t k, const uint32_t *prev, uint32_t *ou
     } else {
         const uint32_t log_chunks = m.d - 6;
         if (cudaError_t e = cudaMemsetAsync(pl->d_keys.p, 0xFF, nent * 8, pl->stream); e != cudaSuccess) {
-            if (capture) {  // do not leave the stream in capture mode
-                cudaGraph_t dead = nullptr;
-                cudaStreamEndCapture(pl->stream, &dead);
-                if (dead) cudaGraphDestroy(dead);
-            }
+            if (capture) end_capture(pl);
             msg = std::string("cudaMemsetAsync (column sweep): ") + cudaGetErrorString(e);
             return WHMEC_ERR_CUDA;
         }
@@ -1722,7 +1533,7 @@ int column_sweep(whmec_plan *pl, std::string &msg) {
     const uint32_t n = pk.n, T = pk.T;
     if (pl->graph_exec) {
         CUDA_TRY(cudaGraphLaunch(pl->graph_exec, pl->stream));
-        pl->arena_seg = pl->bounded ? (uint32_t)pl->seg_col.size() - 2 : 0;
+        pl->arena_seg = pl->col.bounded ? (uint32_t)pl->col.seg_col.size() - 2 : 0;
         return WHMEC_OK;
     }
     const bool capture = pl->sweeps_done >= 1 && n >= 64;
@@ -1733,15 +1544,11 @@ int column_sweep(whmec_plan *pl, std::string &msg) {
     for (uint32_t k = 0; k < n; ++k) {
         int rc = column_launch(pl, k, pl->d_val[curb ^ 1].p, pl->d_val[curb].p, capture, launches, msg);
         if (rc != WHMEC_OK) return rc;
-        if (pl->bounded && next_cut + 1 < pl->seg_col.size() && k + 1 == pl->seg_col[next_cut]) {
+        if (pl->col.bounded && next_cut + 1 < pl->col.seg_col.size() && k + 1 == pl->col.seg_col[next_cut]) {
             const size_t bytes = ((size_t)1 << pk.cols[k].f) * T * 4;
-            cudaError_t e = cudaMemcpyAsync(pl->d_ckpt.p + pl->seg_ckpt[next_cut], pl->d_val[curb].p, bytes, cudaMemcpyDeviceToDevice, pl->stream);
+            cudaError_t e = cudaMemcpyAsync(pl->d_ckpt.p + pl->col.seg_ckpt[next_cut], pl->d_val[curb].p, bytes, cudaMemcpyDeviceToDevice, pl->stream);
             if (e != cudaSuccess) {
-                if (capture) {
-                    cudaGraph_t dead = nullptr;
-                    cudaStreamEndCapture(pl->stream, &dead);
-                    if (dead) cudaGraphDestroy(dead);
-                }
+                if (capture) end_capture(pl);
                 msg = std::string("cudaMemcpyAsync (checkpoint): ") + cudaGetErrorString(e);
                 return WHMEC_ERR_CUDA;
             }
@@ -1750,7 +1557,7 @@ int column_sweep(whmec_plan *pl, std::string &msg) {
         curb ^= 1;
     }
     pl->last_buf = curb ^ 1;
-    if (pl->bounded) pl->arena_seg = (uint32_t)pl->seg_col.size() - 2;
+    if (pl->col.bounded) pl->arena_seg = (uint32_t)pl->col.seg_col.size() - 2;
     pl->stats.kernel_launches = launches;
     if (capture) {
         cudaGraph_t graph = nullptr;
@@ -1777,8 +1584,8 @@ int plan_sweep_impl(whmec_plan *pl, std::string &msg, bool wait = true) {
         rc = pl->tiles.sweep(pl->pk, pl->stream, msg);
         pl->stats.kernel_launches = pl->tiles.launches;
         pl->stats.state_bytes = pl->tiles.state_bytes;
-    } else if (pl->use_ped_batch) {
-        rc = ped_batched_sweep(pl, msg);
+    } else if (pl->col.two_pass()) {
+        rc = ped_two_pass_sweep(pl, msg);
     } else {
         rc = column_sweep(pl, msg);
     }
@@ -1796,7 +1603,7 @@ int plan_sweep_impl(whmec_plan *pl, std::string &msg, bool wait = true) {
 
 BtArgs bt_args(const whmec_plan *pl, int entry) {
     const Packed &pk = pl->pk;
-    return BtArgs{pl->d_cols.p, pl->d_arena.p, pl->d_chain_begin.p, pl->use_ped_batch ? pl->d_last_vals : pl->d_val[pl->last_buf].p,
+    return BtArgs{pl->d_cols.p, pl->d_arena.p, pl->d_chain_begin.p, pl->col.two_pass() ? pl->d_last_vals : pl->d_val[pl->last_buf].p,
                   pk.T, pk.tb, (uint32_t)pk.chain_begin.size() - 1, entry};
 }
 
@@ -1833,14 +1640,14 @@ int bounded_backtrace(whmec_plan *pl, std::string &msg) {
     const Packed &pk = pl->pk;
     uint32_t launches = 0;
     int rc = WHMEC_OK;
-    if (!pl->seg_chain.empty()) {
-        const uint32_t S = (uint32_t)pl->seg_chain.size() - 1;
+    if (!pl->col.seg_chain.empty()) {
+        const uint32_t S = (uint32_t)pl->col.seg_chain.size() - 1;
         for (uint32_t sg = S; sg-- > 0;) {
             if (pl->arena_seg != sg && (rc = ped_segment_pass(pl, sg, launches, msg)) != WHMEC_OK) return rc;
-            const uint32_t c0 = pl->seg_chain[sg];
+            const uint32_t c0 = pl->col.seg_chain[sg];
             BtArgs a = bt_args(pl, sg + 1 == S ? -1 : 0);
             a.chain_begin += c0;
-            a.n_chains = pl->seg_chain[sg + 1] - c0;
+            a.n_chains = pl->col.seg_chain[sg + 1] - c0;
             bt_exits_kernel<<<a.n_chains * a.T, 32, 0, pl->stream>>>(a, pl->d_bt_exits.p);
             bt_entries_kernel<<<1, 32, 0, pl->stream>>>(a, pl->d_bt_exits.p, pl->d_bt_entries.p, nullptr, pl->d_bt_state.p);
             bt_paths_kernel<<<a.n_chains, 32, 0, pl->stream>>>(a, pl->d_bt_entries.p, pl->d_path_index.p, pl->d_path_tv.p,
@@ -1848,13 +1655,13 @@ int bounded_backtrace(whmec_plan *pl, std::string &msg) {
             CUDA_TRY(cudaGetLastError());
         }
     } else {
-        const uint32_t S = (uint32_t)pl->seg_col.size() - 1;
+        const uint32_t S = (uint32_t)pl->col.seg_col.size() - 1;
         const BtView v{pl->d_cols.p, pl->d_arena.p, pk.T, pk.tb};
         for (uint32_t sg = S; sg-- > 0;) {
-            const uint32_t k0 = pl->seg_col[sg], k1 = pl->seg_col[sg + 1];
+            const uint32_t k0 = pl->col.seg_col[sg], k1 = pl->col.seg_col[sg + 1];
             if (pl->arena_seg != sg) {
                 for (uint32_t k = k0; k < k1; ++k) {
-                    const uint32_t *prev = k == k0 && sg ? pl->d_ckpt.p + pl->seg_ckpt[sg] : pl->d_val[(k & 1) ^ 1].p;
+                    const uint32_t *prev = k == k0 && sg ? pl->d_ckpt.p + pl->col.seg_ckpt[sg] : pl->d_val[(k & 1) ^ 1].p;
                     if ((rc = column_launch(pl, k, prev, pl->d_val[k & 1].p, false, launches, msg)) != WHMEC_OK) return rc;
                 }
                 pl->arena_seg = sg;
@@ -1898,8 +1705,8 @@ int plan_finish_impl(whmec_plan *pl, whmec_solution *s, std::string &msg, int en
         CUDA_TRY(cudaMemsetAsync(pl->d_path_tv.p, 0, (size_t)n * 4, pl->stream));
     } else {
         const uint32_t n_chains = (uint32_t)pk.chain_begin.size() - 1;
-        const uint32_t *last_vals = pl->use_ped_batch ? pl->d_last_vals : pl->d_val[pl->last_buf].p;
-        if (pl->bounded) {
+        const uint32_t *last_vals = pl->col.two_pass() ? pl->d_last_vals : pl->d_val[pl->last_buf].p;
+        if (pl->col.bounded) {
             int rc = bounded_backtrace(pl, msg);
             if (rc != WHMEC_OK) return rc;
         } else if (pk.T == 1) {
@@ -1932,7 +1739,7 @@ int plan_finish_impl(whmec_plan *pl, whmec_solution *s, std::string &msg, int en
 
 // ---- segments of a pedigree table (include/whmec.h) ----
 int segment_check(const whmec_plan *pl, std::string &msg) {
-    if (!pl || !pl->segment || !pl->use_ped_batch) {
+    if (!pl || !pl->segment || !pl->col.two_pass()) {
         msg = "not a segment plan (use whmec_segment_create)";
         return WHMEC_ERR_INPUT;
     }
@@ -1947,7 +1754,7 @@ int segment_transfer_impl(whmec_plan *pl, uint32_t *matrix, std::string &msg) {
     CUDA_TRY(cudaSetDevice(pl->device));
     CUDA_TRY(cudaEventRecord(pl->ev0, pl->stream));
     uint32_t launches = 0;
-    if (pl->use_ped_fused) {
+    if (pl->col.path == ColPath::fused) {
         rc = ped_fused_pass(pl, true, msg);
         if (rc == WHMEC_OK) rc = ped_fused_prefix(pl, nullptr, pl->d_matrix.p, msg);
         if (rc != WHMEC_OK) return rc;
@@ -1955,7 +1762,7 @@ int segment_transfer_impl(whmec_plan *pl, uint32_t *matrix, std::string &msg) {
     } else {
         rc = ped_pass(pl, 0, launches, msg);
         if (rc != WHMEC_OK) return rc;
-        ped_prefix_kernel<<<(pk.T + 31) / 32, 32, 0, pl->stream>>>(pl->d_ped_vals.p, pl->ped_max_ent, pk.T, C, pl->d_chain_len.p, nullptr,
+        ped_prefix_kernel<<<(pk.T + 31) / 32, 32, 0, pl->stream>>>(pl->d_ped_vals.p, pl->col.max_ent, pk.T, C, pl->d_chain_len.p, nullptr,
                                                                     pl->segment == 2, pl->d_matrix.p);
         ++launches;
     }
@@ -1985,7 +1792,7 @@ int segment_sweep_impl(whmec_plan *pl, const uint32_t *in_vec, uint32_t *out_vec
     CUDA_TRY(cudaEventRecord(pl->ev0, pl->stream));
     if (in_vec) CUDA_TRY(cudaMemcpyAsync(pl->d_in_vec.p, in_vec, (size_t)T * 4, cudaMemcpyHostToDevice, pl->stream));
     uint32_t launches = 0;
-    if (pl->use_ped_fused) {
+    if (pl->col.path == ColPath::fused) {
         rc = ped_fused_prefix(pl, in_vec ? pl->d_in_vec.p : nullptr, nullptr, msg);
         if (rc == WHMEC_OK) rc = ped_fused_pass(pl, false, msg);
         launches = 2;
@@ -2113,12 +1920,13 @@ int whmec_device_count(void) {
     return n;
 }
 
-static int plan_create_guarded(const whmec_problem *p, int device, whmec_plan **out, char *err, size_t errlen, bool bounded_t1) {
+// segment: see whmec_plan::segment
+static int plan_create_guarded(const whmec_problem *p, int device, whmec_plan **out, char *err, size_t errlen, int segment) {
     return guarded(err, errlen, [&]() -> int {
         std::string msg;
         *out = nullptr;
         std::unique_ptr<whmec_plan> pl(new whmec_plan());  // released (device buffers too) if anything below throws
-        const int rc = plan_create_impl(p, device, pl.get(), msg, 0, bounded_t1);
+        const int rc = plan_create_impl(p, device, pl.get(), msg, segment);
         if (rc != WHMEC_OK) {
             set_err(err, errlen, msg);
             return rc;
@@ -2129,7 +1937,7 @@ static int plan_create_guarded(const whmec_problem *p, int device, whmec_plan **
 }
 
 int whmec_plan_create(const whmec_problem *p, int device, whmec_plan **out, char *err, size_t errlen) {
-    return plan_create_guarded(p, device, out, err, errlen, false);
+    return plan_create_guarded(p, device, out, err, errlen, 0);
 }
 
 int whmec_plan_sweep(whmec_plan *plan, char *err, size_t errlen) {
@@ -2158,18 +1966,7 @@ int whmec_plan_stats(const whmec_plan *plan, whmec_stats *st) {
 void whmec_plan_destroy(whmec_plan *plan) { delete plan; }
 
 int whmec_segment_create(const whmec_problem *p, int device, int continues, whmec_plan **out, char *err, size_t errlen) {
-    return guarded(err, errlen, [&]() -> int {
-        std::string msg;
-        *out = nullptr;
-        std::unique_ptr<whmec_plan> pl(new whmec_plan());
-        const int rc = plan_create_impl(p, device, pl.get(), msg, continues ? 2 : 1);
-        if (rc != WHMEC_OK) {
-            set_err(err, errlen, msg);
-            return rc;
-        }
-        *out = pl.release();
-        return WHMEC_OK;
-    });
+    return plan_create_guarded(p, device, out, err, errlen, continues ? 2 : 1);
 }
 
 int whmec_segment_transfer(whmec_plan *plan, uint32_t *matrix, char *err, size_t errlen) {
@@ -2235,9 +2032,11 @@ static int solve_impl(const whmec_problem *p, whmec_solution *s, int device, whm
             }
         }
     }
-    whmec_plan *pl = nullptr;
-    int rc = whmec_plan_create(p, device, &pl, err, errlen);
-    if (rc == WHMEC_ERR_UNSUPPORTED && err && std::strstr(err, "exceeds the free HBM")) {
+    std::unique_ptr<whmec_plan> pl(new whmec_plan());
+    std::string msg;
+    int rc = plan_create_impl(p, device, pl.get(), msg);
+    if (rc == WHMEC_ERR_UNSUPPORTED && (pl->col.over_hbm || pl->tiles.over_hbm)) {
+        pl.reset();  // (its device buffers go back before the groups are planned)
         // the back-pointers of the whole table do not fit: chains of a single individual are independent problems,
         // solve them group after group (2, 4, ... groups until a group fits)
         for (uint32_t G = 2; G <= 1024; G *= 2) {
@@ -2248,22 +2047,25 @@ static int solve_impl(const whmec_problem *p, whmec_solution *s, int device, whm
             solve_in_groups(p, s, G, be, msg, &handled);
             if (handled) {
                 if (st) *st = be.inner.total;
-                if (errlen) err[0] = 0;
                 return WHMEC_OK;
             }
         }
         // no group fits (one chain alone is too large): the memory-bounded sweep of the whole table
-        rc = plan_create_guarded(p, device, &pl, err, errlen, true);
+        pl.reset(new whmec_plan());
+        rc = plan_create_impl(p, device, pl.get(), msg, 0, true);
     }
-    if (rc != WHMEC_OK) return rc;
+    if (rc != WHMEC_OK) {
+        set_err(err, errlen, msg);
+        return rc;
+    }
     const auto t1 = clk::now();
-    rc = whmec_plan_sweep(pl, err, errlen);
+    rc = whmec_plan_sweep(pl.get(), err, errlen);
     const auto t2 = clk::now();
-    if (rc == WHMEC_OK) rc = whmec_plan_finish(pl, s, err, errlen);
+    if (rc == WHMEC_OK) rc = whmec_plan_finish(pl.get(), s, err, errlen);
     const auto t3 = clk::now();
     const whmec_stats stats = pl->stats;
     if (st) *st = stats;
-    whmec_plan_destroy(pl);
+    pl.reset();
     if (timing)
         std::fprintf(stderr, "[whmec] solve: create %.2f ms (h2d %.2f), sweep %.2f ms (device %.2f), finish %.2f ms (device %.2f), destroy %.2f ms\n",
                      ms(t0, t1), (double)stats.h2d_ms, ms(t1, t2), (double)stats.sweep_ms, ms(t2, t3), (double)stats.d2h_ms, ms(t3, clk::now()));
