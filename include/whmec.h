@@ -184,6 +184,35 @@ int whmec_segment_sweep(whmec_plan *plan, const uint32_t *in_vec /* [T] or NULL 
 int whmec_segment_exits(whmec_plan *plan, int is_last, uint32_t *exits /* [T] */, char *err, size_t errlen);
 int whmec_segment_finish(whmec_plan *plan, int entry, whmec_solution *s, char *err, size_t errlen);
 
+/* ---- A pedigree table (T = 4^trios > 1) genotyped by several GPUs -----------------------------
+ * whmec_genotype sweeps a family's forward-backward table column by column on one device.  A SEGMENT is a run of whole chains
+ * given as a problem of its own (as for whmec_segment_*: its columns, its reads, its priors, recombcost of exactly these
+ * columns).  Only the T values of the cut cross between segments, and both recursions are linear in them: a segment's
+ * forward output is alpha . M for a T x T transfer matrix M.  The caller (whatshap_b200/multigpu.py) moves T x T double
+ * matrices and T-vectors between the processes:
+ *   1. whmec_genotype_segment_create   pack + upload; `continues` != 0 unless the segment starts the table, `continued` != 0
+ *                                      unless it ends the table
+ *   2. whmec_genotype_segment_transfer matrix[u*T + i] = forward value at transmission value i of the segment's last column when
+ *                                      the vector handed to it is e_u (the table's last segment: the total mass at i); the
+ *                                      first segment ignores its input: all rows equal.  One positive factor on the whole
+ *                                      matrix is left open (it cancels in the normalisation)
+ *   3. (caller) all-gather the matrices and fold them: alpha_1 = M_0[0], alpha_{s+1} = alpha_s . M_s (left to right),
+ *      beta_{S-2} = M_{S-1} . 1, beta_s = M_{s+1} . beta_{s+1} (right to left), each divided by its largest entry
+ *   4. whmec_genotype_segment_run      the backward and forward passes of the segment from its true inputs: alpha_in (iff
+ *                                      continues) is the forward vector in front of it, beta_in (iff continued) the backward
+ *                                      vector behind it; likelihoods [n_ind][segment columns][3] as whmec_genotype's
+ * The likelihoods agree with whmec_genotype on the whole table to ~1e-14.  A segment whose backward tables do not fit runs in
+ * memory-bounded mode, like a table of whmec_genotype.  st (optional) receives the pass's device time and launches.
+ * WHMEC_ERR_UNSUPPORTED: single-individual problems (their chains are independent tables; shard them with whmec_genotype);
+ * WHMEC_ERR_INPUT: a missing alpha_in / beta_in. */
+typedef struct whmec_gl_segment whmec_gl_segment;
+int whmec_genotype_segment_create(const whmec_problem *p, int device, int continues, int continued, whmec_gl_segment **out, char *err,
+                                  size_t errlen);
+int whmec_genotype_segment_transfer(whmec_gl_segment *s, double *matrix /* [T*T] */, whmec_stats *st_or_null, char *err, size_t errlen);
+int whmec_genotype_segment_run(whmec_gl_segment *s, const double *alpha_in /* [T] iff continues */, const double *beta_in /* [T] iff continued */,
+                               double *likelihoods /* [n_ind][n_cols][3] */, whmec_stats *st_or_null, char *err, size_t errlen);
+void whmec_genotype_segment_destroy(whmec_gl_segment *s);
+
 /* ---- Coverage-capping read selection (host only; the step before the DP) -------------------------
  * whatshap/readselect.pyx:240-272 picks reads greedily by score until every variant is covered or max_cov
  * is reached.  Which read wins a tie is decided by the sift rules of the reference's positional max-heap

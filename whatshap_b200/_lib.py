@@ -42,6 +42,10 @@ EXPORTS = (
     "whmec_selector_bridge",
     "whmec_read_sort_key",
     "whmec_genotype",
+    "whmec_genotype_segment_create",
+    "whmec_genotype_segment_transfer",
+    "whmec_genotype_segment_run",
+    "whmec_genotype_segment_destroy",
     "whmec_compute_genotypes",
     "whmec_heuristic",
 )
@@ -101,6 +105,14 @@ def lib() -> C.CDLL:
     L.whmec_segment_sweep.argtypes = [C.c_void_p, u32p, u32p, C.c_char_p, C.c_size_t]
     L.whmec_segment_exits.argtypes = [C.c_void_p, C.c_int, u32p, C.c_char_p, C.c_size_t]
     L.whmec_segment_finish.argtypes = [C.c_void_p, C.c_int, C.POINTER(CSolution), C.c_char_p, C.c_size_t]
+    f64p = C.POINTER(C.c_double)
+    L.whmec_genotype_segment_create.argtypes = [C.POINTER(CProblem), C.c_int, C.c_int, C.c_int, C.POINTER(C.c_void_p), C.c_char_p, C.c_size_t]
+    L.whmec_genotype_segment_transfer.argtypes = [C.c_void_p, f64p, C.POINTER(CStats), C.c_char_p, C.c_size_t]
+    L.whmec_genotype_segment_run.argtypes = [C.c_void_p, f64p, f64p, f64p, C.POINTER(CStats), C.c_char_p, C.c_size_t]
+    L.whmec_genotype_segment_destroy.argtypes = [C.c_void_p]
+    L.whmec_genotype_segment_destroy.restype = None
+    for name in ("whmec_genotype_segment_create", "whmec_genotype_segment_transfer", "whmec_genotype_segment_run"):
+        getattr(L, name).restype = C.c_int
     for name in ("whmec_plan_create", "whmec_plan_sweep", "whmec_plan_finish", "whmec_plan_stats", "whmec_solve",
                  "whmec_segment_create", "whmec_segment_transfer", "whmec_segment_sweep", "whmec_segment_exits",
                  "whmec_segment_finish"):
@@ -259,6 +271,56 @@ class Segment:
     def close(self) -> None:
         if self._h:
             lib().whmec_plan_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class GenotypeSegment:
+    """A run of whole chains of a pedigree genotyping table on one GPU (`whmec_genotype_segment_*`, include/whmec.h): the unit
+    `multigpu.genotype_sharded` spreads over the ranks when T > 1.  `continues`: the segment does not start the table;
+    `continued`: it does not end it.  `stats` holds the statistics of the last `transfer()` / `run()`."""
+
+    def __init__(self, prob: FlatProblem, continues: bool, continued: bool, device: int = 0):
+        self.prob = prob
+        self.T = 4 ** prob.n_trios
+        self.stats: dict = {}
+        self._h = C.c_void_p()
+        cp = prob.as_c()
+        err = C.create_string_buffer(512)
+        rc = lib().whmec_genotype_segment_create(C.byref(cp), device, int(bool(continues)), int(bool(continued)), C.byref(self._h), err, len(err))
+        raise_for(rc, err.value.decode())
+
+    @staticmethod
+    def _ptr(a):
+        return None if a is None else a.ctypes.data_as(C.POINTER(C.c_double))
+
+    def transfer(self) -> np.ndarray:
+        """The T x T transfer matrix: row u is the segment's forward output for the input e_u."""
+        m = np.zeros((self.T, self.T), np.float64)
+        st, err = CStats(), C.create_string_buffer(512)
+        raise_for(lib().whmec_genotype_segment_transfer(self._h, self._ptr(m), C.byref(st), err, len(err)), err.value.decode())
+        self.stats = st.as_dict()
+        return m
+
+    def run(self, alpha: Optional[np.ndarray] = None, beta: Optional[np.ndarray] = None) -> np.ndarray:
+        """Likelihoods [n_ind, segment columns, 3] from the true forward input `alpha` and backward input `beta` (T each)."""
+        out = np.zeros((self.prob.n_ind, self.prob.n_cols, 3), np.float64)
+        a = None if alpha is None else np.ascontiguousarray(alpha, np.float64)
+        b = None if beta is None else np.ascontiguousarray(beta, np.float64)
+        st, err = CStats(), C.create_string_buffer(512)
+        raise_for(lib().whmec_genotype_segment_run(self._h, self._ptr(a), self._ptr(b), self._ptr(out), C.byref(st), err, len(err)),
+                  err.value.decode())
+        self.stats = st.as_dict()
+        return out
+
+    def close(self) -> None:
+        if self._h:
+            lib().whmec_genotype_segment_destroy(self._h)
             self._h = C.c_void_p()
 
     def __del__(self):

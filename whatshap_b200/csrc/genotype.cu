@@ -11,12 +11,16 @@
 // memory-bounded mode (gl_bounded, DESIGN §4.5): its columns are cut into segments that share one arena, and every
 // segment but the first is swept backward again from a checkpoint before its forward steps (the reference keeps every
 // sqrt(n)-th column and recomputes, genotypedptable.cpp:139-166,326-343).
+// A pedigree table can also be split into segments of whole chains, one per GPU (whmec_genotype_segment_*, DESIGN §4.5): a
+// forward-only transfer pass per segment (gl_transfer_kernel) gives the T x T matrix that carries the T values across the
+// cut, the caller folds the matrices, and each segment runs the passes above from its true inputs.
 #include <cuda_runtime.h>
 
 #include <algorithm>
 #include <chrono>
 #include <cstdlib>
 #include <cstring>
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -100,8 +104,36 @@ __global__ void __launch_bounds__(1024) gl_scale_kernel(const GlStep *steps, dou
     for (uint64_t i = threadIdx.x; i < st.n_clear; i += blockDim.x) c[i] = 0.0;
 }
 
+// Transfer pass of a segment (gl_transfer_plan): one column for the n_in input rows of a batch.  grid.x covers the column.
+__global__ void __launch_bounds__(GL_THREADS) gl_transfer_kernel(GlView v, const GlStep *step, double *F, uint32_t n_in) {
+    const GlStep st = *step;
+    const uint64_t x = (uint64_t)blockIdx.x * GL_THREADS + threadIdx.x;
+    if (x >= ((uint64_t)1 << st.cells_log2)) return;
+    gl_transfer_cell(v, st.k, (uint32_t)x, n_in, F + st.prev_off, F + st.cur_off, AtomicAdd());
+}
+
+// Writes the largest entry of the finished column (pool + cur_off, n_scale entries; 0 when all are 0) to *col_max, before
+// gl_scale_kernel divides by it: the transfer pass of a segment with several batches puts their rows on one scale with these
+// (gl_transfer_combine).
+__global__ void __launch_bounds__(1024) gl_column_max_kernel(const GlStep *step, const double *pool, double *col_max) {
+    __shared__ double s_max[32];
+    const GlStep st = *step;
+    const double *v = pool + st.cur_off;
+    double mx = 0.0;
+    for (uint64_t i = threadIdx.x; i < st.n_scale; i += blockDim.x) mx = fmax(mx, v[i]);
+    for (int off = 16; off > 0; off >>= 1) mx = fmax(mx, __shfl_down_sync(0xFFFFFFFFu, mx, off));
+    if ((threadIdx.x & 31) == 0) s_max[threadIdx.x >> 5] = mx;
+    __syncthreads();
+    if (threadIdx.x < 32) {
+        mx = threadIdx.x < (blockDim.x >> 5) ? s_max[threadIdx.x] : 0.0;
+        for (int off = 16; off > 0; off >>= 1) mx = fmax(mx, __shfl_down_sync(0xFFFFFFFFu, mx, off));
+        if (threadIdx.x == 0) *col_max = mx;
+    }
+}
+
 struct Buffers {  // freed on every exit path
     cudaStream_t stream = nullptr;
+    bool owns_stream = true;  // false: the stream belongs to a longer-lived Buffers
     std::vector<void *> ptrs;
     template <class Tp>
     cudaError_t alloc(Tp **p, size_t count) {
@@ -113,60 +145,17 @@ struct Buffers {  // freed on every exit path
         for (void *p : ptrs) cudaFreeAsync(p, stream);
         if (stream) {
             cudaStreamSynchronize(stream);
-            cudaStreamDestroy(stream);
+            if (owns_stream) cudaStreamDestroy(stream);
         }
     }
 };
 
-int genotype_impl(const whmec_problem *p, double *likelihoods, int device, whmec_stats *st, std::string &msg) {
-    if (!p || !likelihoods) {
-        msg = "null argument";
-        return WHMEC_ERR_INPUT;
-    }
-    Packed pk;
-    GlPacked g;
-    int rc = gl_pack(p, pk, g, msg);
-    if (rc != WHMEC_OK) return rc;
-    if (st) *st = pk.stats;
-    const uint32_t n = pk.n, T = pk.T, n_ind = pk.n_ind;
-    if (n == 0) return WHMEC_OK;
-    int n_dev = 0;
-    if (cudaGetDeviceCount(&n_dev) != cudaSuccess || n_dev == 0) {
-        msg = "no CUDA device (whatshap_b200 has no CPU path)";
-        return WHMEC_ERR_CUDA;
-    }
-    CUDA_TRY(cudaSetDevice(device));
-    Buffers B;
-    CUDA_TRY(cudaStreamCreateWithFlags(&B.stream, cudaStreamNonBlocking));
+// The packed problem in HBM: per-column records, error probabilities, alleles, pedigree indices, transition and prior tables.
+int upload_inputs(Buffers &B, const Packed &pk, const GlPacked &g, GlView &v, uint64_t &h2d, std::string &msg) {
+    const uint32_t n = pk.n;
     cudaStream_t s = B.stream;
-
-    // groups of whole tables (T == 1: chains; otherwise the one table) whose backward tables fit the device together
-    const size_t free_b = device_available_bytes();
-    const uint64_t fixed = (uint64_t)n * sizeof(GlCol) + g.eps.size() * 10 + (g.trans.size() + g.q.size()) * 8 + (uint64_t)n * sizeof(GlStep) * 2 +
-                           (uint64_t)n * n_ind * 3 * 8 + (512ull << 20);
-    if (fixed > free_b) {
-        msg = "genotyping: problem exceeds the free HBM of this device";
-        return WHMEC_ERR_UNSUPPORTED;
-    }
-    uint64_t budget = (free_b - fixed) / 8;  // doubles available for backward tables + projection buffers
-    // WHMEC_GENOTYPE_ARENA_BUDGET=bytes (test hook): the budget for backward tables, checkpoints and projection buffers
-    if (const char *e = std::getenv("WHMEC_GENOTYPE_ARENA_BUDGET")) budget = std::min<uint64_t>(budget, std::strtoull(e, nullptr, 10) / 8);
-    // groups of tables on launch schedules (one launch advances every table of a group by one column); a table whose
-    // backward tables do not fit runs alone in memory-bounded mode (gl_bounded)
-    std::vector<GlUnit> units;
-    rc = gl_plan(g, T, budget, units, msg);
-    if (rc != WHMEC_OK) return rc;
-    uint64_t max_work = 1, max_steps = 1, max_store = 0;  // max_store: the largest backward store of a unit (doubles)
-    bool bounded = false;
-    for (const GlUnit &u : units) {
-        max_work = std::max(max_work, u.work_doubles);
-        max_steps = std::max<uint64_t>(max_steps, u.bounded ? u.bd.steps.size() : u.sc.steps.size());
-        max_store = std::max(max_store, u.bounded ? u.bd.arena_doubles + u.bd.ckpt_doubles : u.sc.beta_doubles);
-        bounded = bounded || u.bounded;
-    }
     GlCol *d_cols = nullptr;
-    double *d_eps = nullptr, *d_trans = nullptr, *d_q = nullptr, *d_work = nullptr, *d_acc = nullptr;
-    GlStep *d_steps = nullptr;
+    double *d_eps = nullptr, *d_trans = nullptr, *d_q = nullptr;
     uint8_t *d_allele = nullptr, *d_ind = nullptr;
     int8_t *d_h2p = nullptr;
     CUDA_TRY(B.alloc(&d_cols, n));
@@ -176,10 +165,6 @@ int genotype_impl(const whmec_problem *p, double *likelihoods, int device, whmec
     CUDA_TRY(B.alloc(&d_h2p, pk.h2p.size()));
     CUDA_TRY(B.alloc(&d_trans, g.trans.size()));
     CUDA_TRY(B.alloc(&d_q, g.q.size()));
-    CUDA_TRY(B.alloc(&d_work, max_work));  // per unit: its backward store, then its projection buffers
-    CUDA_TRY(B.alloc(&d_steps, max_steps));
-    CUDA_TRY(B.alloc(&d_acc, (size_t)n * n_ind * 3));
-    uint64_t h2d = 0;
     auto up = [&](void *dst, const void *src, size_t bytes) {
         h2d += bytes;
         return bytes ? cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, s) : cudaSuccess;
@@ -191,14 +176,42 @@ int genotype_impl(const whmec_problem *p, double *likelihoods, int device, whmec
     CUDA_TRY(up(d_h2p, pk.h2p.data(), pk.h2p.size()));
     CUDA_TRY(up(d_trans, g.trans.data(), g.trans.size() * 8));
     CUDA_TRY(up(d_q, g.q.data(), g.q.size() * 8));
-    CUDA_TRY(cudaMemsetAsync(d_acc, 0, (size_t)n * n_ind * 3 * 8, s));
-    const GlView v{d_cols, d_eps, d_allele, d_ind, d_h2p, d_trans, d_q, T, pk.P, n_ind};
+    v = GlView{d_cols, d_eps, d_allele, d_ind, d_h2p, d_trans, d_q, pk.T, pk.P, pk.n_ind};
+    return WHMEC_OK;
+}
 
-    cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-    CUDA_TRY(cudaEventCreate(&ev0));
-    CUDA_TRY(cudaEventCreate(&ev1));
-    CUDA_TRY(cudaEventRecord(ev0, s));
-    uint32_t launches = 0;
+// Bytes the inputs above and the per-call arrays take; the budget for backward tables + projection buffers is what remains of
+// the free HBM (or WHMEC_GENOTYPE_ARENA_BUDGET, whichever is smaller), in doubles.
+int work_budget(const Packed &pk, const GlPacked &g, uint64_t &budget, std::string &msg) {
+    const uint32_t n = pk.n, n_ind = pk.n_ind;
+    const size_t free_b = device_available_bytes();
+    const uint64_t fixed = (uint64_t)n * sizeof(GlCol) + g.eps.size() * 10 + (g.trans.size() + g.q.size()) * 8 + (uint64_t)n * sizeof(GlStep) * 2 +
+                           (uint64_t)n * n_ind * 3 * 8 + (512ull << 20);
+    if (fixed > free_b) {
+        msg = "genotyping: problem exceeds the free HBM of this device";
+        return WHMEC_ERR_UNSUPPORTED;
+    }
+    budget = (free_b - fixed) / 8;  // doubles available for backward tables + projection buffers
+    // WHMEC_GENOTYPE_ARENA_BUDGET=bytes (test hook): the budget for backward tables, checkpoints and projection buffers
+    if (const char *e = std::getenv("WHMEC_GENOTYPE_ARENA_BUDGET")) budget = std::min<uint64_t>(budget, std::strtoull(e, nullptr, 10) / 8);
+    return WHMEC_OK;
+}
+
+// Runs the units of gl_plan on stream s, accumulating the posteriors into d_acc ([n_cols][n_ind * 3]).  d_work holds the largest
+// unit's work_doubles (per unit: its backward store, then its projection buffers), d_steps its step list.  A segment of a table
+// passes alpha_in / beta_in (T doubles each, or null), which go where the unit's plan says (GlUnit::alpha_at, beta_at).
+int run_units(cudaStream_t s, const GlView &v, const std::vector<GlUnit> &units, const double *alpha_in, const double *beta_in, double *d_work,
+              GlStep *d_steps, double *d_acc, uint32_t &launches, uint64_t &h2d, std::string &msg) {
+    auto up = [&](void *dst, const void *src, size_t bytes) {
+        h2d += bytes;
+        return bytes ? cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, s) : cudaSuccess;
+    };
+    auto inputs = [&](const GlUnit &u) {  // after the unit's buffers are cleared
+        cudaError_t e = cudaSuccess;
+        if (alpha_in) e = up(d_work + u.alpha_at, alpha_in, (size_t)v.T * 8);
+        if (e == cudaSuccess && beta_in) e = up(d_work + u.beta_at, beta_in, (size_t)v.T * 8);
+        return e;
+    };
     constexpr uint32_t MAX_GRID_Y = 65535;
     for (size_t q = 0; q < units.size(); ++q) {
         if (q > 0) CUDA_TRY(cudaStreamSynchronize(s));  // the step list of the previous unit is still being read
@@ -208,6 +221,7 @@ int genotype_impl(const whmec_problem *p, double *likelihoods, int device, whmec
             double *d_beta = d_work, *d_F = d_work + store;
             CUDA_TRY(up(d_steps, bd.steps.data(), bd.steps.size() * sizeof(GlStep)));
             CUDA_TRY(cudaMemsetAsync(d_work, 0, (store + bd.f_pool_doubles) * 8, s));
+            CUDA_TRY(inputs(units[q]));
             auto blocks = [&](uint32_t e) { return (unsigned)((((uint64_t)1 << bd.steps[e].cells_log2) + GL_THREADS - 1) / GL_THREADS); };
             for (const GlSweep &sw : bd.sweeps) {
                 if (sw.clear) CUDA_TRY(cudaMemsetAsync(d_beta, 0, sw.clear * 8, s));
@@ -230,6 +244,7 @@ int genotype_impl(const whmec_problem *p, double *likelihoods, int device, whmec
         CUDA_TRY(up(d_steps, sc.steps.data(), sc.steps.size() * sizeof(GlStep)));
         CUDA_TRY(cudaMemsetAsync(d_beta, 0, (sc.beta_doubles + 1) * 8, s));
         CUDA_TRY(cudaMemsetAsync(d_F, 0, sc.f_pool_doubles * 8, s));
+        CUDA_TRY(inputs(units[q]));
         auto widest = [&](uint32_t e0, uint32_t e1) {
             uint32_t a_max = 0;
             for (uint32_t e = e0; e < e1; ++e) a_max = std::max(a_max, sc.steps[e].cells_log2);
@@ -250,17 +265,75 @@ int genotype_impl(const whmec_problem *p, double *likelihoods, int device, whmec
                 launches += 2;
             }
     }
+    return WHMEC_OK;
+}
+
+struct Timer {  // CUDA events around the work enqueued between start() and stop()
+    cudaEvent_t ev0 = nullptr, ev1 = nullptr;
+    ~Timer() {
+        if (ev0) cudaEventDestroy(ev0);
+        if (ev1) cudaEventDestroy(ev1);
+    }
+    cudaError_t start(cudaStream_t s) {
+        cudaError_t e = cudaEventCreate(&ev0);
+        if (e == cudaSuccess) e = cudaEventCreate(&ev1);
+        return e == cudaSuccess ? cudaEventRecord(ev0, s) : e;
+    }
+};
+
+int open_device(int device, std::string &msg) {
+    int n_dev = 0;
+    if (cudaGetDeviceCount(&n_dev) != cudaSuccess || n_dev == 0) {
+        msg = "no CUDA device (whatshap_b200 has no CPU path)";
+        return WHMEC_ERR_CUDA;
+    }
+    CUDA_TRY(cudaSetDevice(device));
+    return WHMEC_OK;
+}
+
+// Groups of tables or bounded tables (gl_plan) of one packed problem on the device, posteriors normalised into `likelihoods`.
+// Shared by whmec_genotype (alpha_in = beta_in = null) and whmec_genotype_segment_run.
+int run_packed(Buffers &B, const Packed &pk, const GlPacked &g, const GlView &v, uint64_t budget, const double *alpha_in, const double *beta_in,
+               double *likelihoods, whmec_stats *st, uint64_t h2d, std::string &msg) {
+    const uint32_t n = pk.n, n_ind = pk.n_ind;
+    cudaStream_t s = B.stream;
+    // groups of tables on launch schedules (one launch advances every table of a group by one column); a table whose
+    // backward tables do not fit runs alone in memory-bounded mode (gl_bounded)
+    std::vector<GlUnit> units;
+    int rc = gl_plan(g, pk.T, budget, units, msg);
+    if (rc != WHMEC_OK) return rc;
+    uint64_t max_work = 1, max_steps = 1, max_store = 0;  // max_store: the largest backward store of a unit (doubles)
+    bool bounded = false;
+    for (const GlUnit &u : units) {
+        max_work = std::max(max_work, u.work_doubles);
+        max_steps = std::max<uint64_t>(max_steps, u.bounded ? u.bd.steps.size() : u.sc.steps.size());
+        max_store = std::max(max_store, u.bounded ? u.bd.arena_doubles + u.bd.ckpt_doubles : u.sc.beta_doubles);
+        bounded = bounded || u.bounded;
+    }
+    Buffers W;  // this call's buffers, on the same stream, allocated before the timed region
+    W.stream = s;
+    W.owns_stream = false;
+    double *d_work = nullptr, *d_acc = nullptr;
+    GlStep *d_steps = nullptr;
+    CUDA_TRY(W.alloc(&d_work, max_work));
+    CUDA_TRY(W.alloc(&d_steps, max_steps));
+    CUDA_TRY(W.alloc(&d_acc, (size_t)n * n_ind * 3));
+    CUDA_TRY(cudaMemsetAsync(d_acc, 0, (size_t)n * n_ind * 3 * 8, s));
+    Timer tm;
+    CUDA_TRY(tm.start(s));
+    uint32_t launches = 0;
+    rc = run_units(s, v, units, alpha_in, beta_in, d_work, d_steps, d_acc, launches, h2d, msg);
+    if (rc != WHMEC_OK) return rc;
     CUDA_TRY(cudaGetLastError());
-    CUDA_TRY(cudaEventRecord(ev1, s));
+    CUDA_TRY(cudaEventRecord(tm.ev1, s));
     std::vector<double> acc((size_t)n * n_ind * 3);
     CUDA_TRY(cudaMemcpyAsync(acc.data(), d_acc, acc.size() * 8, cudaMemcpyDeviceToHost, s));
     CUDA_TRY(cudaStreamSynchronize(s));
     float ms = 0.f;
-    CUDA_TRY(cudaEventElapsedTime(&ms, ev0, ev1));
-    cudaEventDestroy(ev0);
-    cudaEventDestroy(ev1);
+    CUDA_TRY(cudaEventElapsedTime(&ms, tm.ev0, tm.ev1));
     gl_normalise(acc.data(), n, n_ind, likelihoods);
     if (st) {
+        *st = pk.stats;
         st->kernel_launches = launches;
         st->sweep_ms = ms;
         st->h2d_bytes = h2d;
@@ -273,13 +346,37 @@ int genotype_impl(const whmec_problem *p, double *likelihoods, int device, whmec
     return WHMEC_OK;
 }
 
-}  // namespace
+int genotype_impl(const whmec_problem *p, double *likelihoods, int device, whmec_stats *st, std::string &msg) {
+    if (!p || !likelihoods) {
+        msg = "null argument";
+        return WHMEC_ERR_INPUT;
+    }
+    Packed pk;
+    GlPacked g;
+    int rc = gl_pack(p, pk, g, msg);
+    if (rc != WHMEC_OK) return rc;
+    if (st) *st = pk.stats;
+    if (pk.n == 0) return WHMEC_OK;
+    rc = open_device(device, msg);
+    if (rc != WHMEC_OK) return rc;
+    Buffers B;
+    CUDA_TRY(cudaStreamCreateWithFlags(&B.stream, cudaStreamNonBlocking));
+    uint64_t budget = 0;
+    rc = work_budget(pk, g, budget, msg);
+    if (rc != WHMEC_OK) return rc;
+    uint64_t h2d = 0;
+    GlView v{};
+    rc = upload_inputs(B, pk, g, v, h2d, msg);
+    if (rc != WHMEC_OK) return rc;
+    return run_packed(B, pk, g, v, budget, nullptr, nullptr, likelihoods, st, h2d, msg);
+}
 
-extern "C" int whmec_genotype(const whmec_problem *p, double *likelihoods, int device, whmec_stats *st, char *err, size_t errlen) {
+template <class F>
+int guarded(F &&fn, char *err, size_t errlen) {
     std::string msg;
     int rc;
     try {
-        rc = genotype_impl(p, likelihoods, device, st, msg);
+        rc = fn(msg);
     } catch (const std::exception &e) {  // no C++ exception crosses the C boundary
         msg = e.what();
         rc = WHMEC_ERR_INPUT;
@@ -289,4 +386,155 @@ extern "C" int whmec_genotype(const whmec_problem *p, double *likelihoods, int d
         err[errlen - 1] = 0;
     }
     return rc;
+}
+
+}  // namespace
+
+// A segment of a pedigree table on one device (include/whmec.h): packed and uploaded once, then the transfer pass and the run.
+struct whmec_gl_segment {
+    int device = 0;
+    bool continues = false, continued = false;
+    Packed pk;
+    GlPacked g;
+    Buffers B;  // the stream and the uploaded inputs
+    GlView v{};
+    uint64_t h2d = 0;
+};
+
+extern "C" int whmec_genotype(const whmec_problem *p, double *likelihoods, int device, whmec_stats *st, char *err, size_t errlen) {
+    return guarded([&](std::string &msg) { return genotype_impl(p, likelihoods, device, st, msg); }, err, errlen);
+}
+
+extern "C" int whmec_genotype_segment_create(const whmec_problem *p, int device, int continues, int continued, whmec_gl_segment **out, char *err,
+                                             size_t errlen) {
+    return guarded(
+        [&](std::string &msg) {
+            if (!p || !out) {
+                msg = "null argument";
+                return WHMEC_ERR_INPUT;
+            }
+            *out = nullptr;
+            auto sg = std::make_unique<whmec_gl_segment>();
+            sg->device = device;
+            sg->continues = continues != 0;
+            sg->continued = continued != 0;
+            int rc = gl_pack_segment(p, sg->continues, sg->continued, sg->pk, sg->g, msg);
+            if (rc != WHMEC_OK) return rc;
+            if (sg->pk.n == 0) {
+                msg = "genotyping segments: a segment needs at least one column";
+                return WHMEC_ERR_INPUT;
+            }
+            rc = open_device(device, msg);
+            if (rc != WHMEC_OK) return rc;
+            CUDA_TRY(cudaStreamCreateWithFlags(&sg->B.stream, cudaStreamNonBlocking));
+            rc = upload_inputs(sg->B, sg->pk, sg->g, sg->v, sg->h2d, msg);
+            if (rc != WHMEC_OK) return rc;
+            CUDA_TRY(cudaStreamSynchronize(sg->B.stream));
+            *out = sg.release();
+            return WHMEC_OK;
+        },
+        err, errlen);
+}
+
+extern "C" int whmec_genotype_segment_transfer(whmec_gl_segment *sg, double *matrix, whmec_stats *st, char *err, size_t errlen) {
+    return guarded(
+        [&](std::string &msg) {
+            if (!sg || !matrix) {
+                msg = "null argument";
+                return WHMEC_ERR_INPUT;
+            }
+            CUDA_TRY(cudaSetDevice(sg->device));
+            const uint32_t T = sg->pk.T, n = sg->pk.n;
+            GlTransfer tp;
+            gl_transfer_plan(sg->g, T, sg->continues, tp);
+            cudaStream_t s = sg->B.stream;
+            Buffers W;
+            W.stream = s;
+            W.owns_stream = false;
+            // the batches' inputs, rows and column scales stay on the device until the timed region is over: no host work
+            // between the batches
+            const size_t batch = (size_t)tp.n_in * T, n_max = tp.n_batches > 1 ? (size_t)tp.n_batches * n : 0;
+            double *d_F = nullptr, *d_in = nullptr, *d_rows = nullptr, *d_max = nullptr;
+            GlStep *d_steps = nullptr;
+            CUDA_TRY(W.alloc(&d_F, tp.f_pool_doubles));
+            CUDA_TRY(W.alloc(&d_steps, n));
+            CUDA_TRY(W.alloc(&d_rows, tp.n_batches * batch));
+            CUDA_TRY(W.alloc(&d_max, n_max));
+            std::vector<double> rows(tp.n_batches * batch), col_max(n_max), inputs;
+            uint64_t h2d = (uint64_t)n * sizeof(GlStep);
+            CUDA_TRY(cudaMemcpyAsync(d_steps, tp.steps.data(), (size_t)n * sizeof(GlStep), cudaMemcpyHostToDevice, s));
+            if (sg->continues) {  // batch b's inputs: e_u for u = b * n_in + r, one row each
+                inputs.assign(tp.n_batches * batch, 0.0);
+                for (uint32_t u = 0; u < tp.n_batches * tp.n_in; ++u) inputs[(size_t)u * T + u] = 1.0;
+                CUDA_TRY(W.alloc(&d_in, inputs.size()));
+                CUDA_TRY(cudaMemcpyAsync(d_in, inputs.data(), inputs.size() * 8, cudaMemcpyHostToDevice, s));
+                h2d += inputs.size() * 8;
+            }
+            Timer tm;
+            CUDA_TRY(tm.start(s));
+            uint32_t launches = 0;
+            for (uint32_t b = 0; b < tp.n_batches; ++b) {
+                CUDA_TRY(cudaMemsetAsync(d_F, 0, tp.f_pool_doubles * 8, s));
+                if (d_in) CUDA_TRY(cudaMemcpyAsync(d_F + tp.in_off, d_in + b * batch, batch * 8, cudaMemcpyDeviceToDevice, s));
+                for (uint32_t k = 0; k < n; ++k) {
+                    const unsigned blocks = (unsigned)((((uint64_t)1 << tp.steps[k].cells_log2) + GL_THREADS - 1) / GL_THREADS);
+                    gl_transfer_kernel<<<blocks, GL_THREADS, 0, s>>>(sg->v, d_steps + k, d_F, tp.n_in);
+                    if (n_max) gl_column_max_kernel<<<1, 1024, 0, s>>>(d_steps + k, d_F, d_max + (size_t)b * n + k);
+                    gl_scale_kernel<<<1, 1024, 0, s>>>(d_steps + k, d_F);
+                    launches += n_max ? 3 : 2;
+                }
+                CUDA_TRY(cudaMemcpyAsync(d_rows + b * batch, d_F + tp.out_off, batch * 8, cudaMemcpyDeviceToDevice, s));
+            }
+            CUDA_TRY(cudaGetLastError());
+            CUDA_TRY(cudaEventRecord(tm.ev1, s));
+            CUDA_TRY(cudaMemcpyAsync(rows.data(), d_rows, rows.size() * 8, cudaMemcpyDeviceToHost, s));
+            if (n_max) CUDA_TRY(cudaMemcpyAsync(col_max.data(), d_max, n_max * 8, cudaMemcpyDeviceToHost, s));
+            CUDA_TRY(cudaStreamSynchronize(s));
+            float ms = 0.f;
+            CUDA_TRY(cudaEventElapsedTime(&ms, tm.ev0, tm.ev1));
+            gl_transfer_combine(tp, T, rows, col_max, matrix);
+            if (st) {
+                *st = sg->pk.stats;
+                st->kernel_launches = launches;
+                st->sweep_ms = ms;
+                st->h2d_bytes = h2d;
+                st->d2h_bytes = (rows.size() + col_max.size()) * 8;
+                st->backptr_bytes = 0;  // no backward tables in this pass
+                st->path_kind = 4;
+            }
+            return WHMEC_OK;
+        },
+        err, errlen);
+}
+
+extern "C" int whmec_genotype_segment_run(whmec_gl_segment *sg, const double *alpha_in, const double *beta_in, double *likelihoods, whmec_stats *st,
+                                          char *err, size_t errlen) {
+    return guarded(
+        [&](std::string &msg) {
+            if (!sg || !likelihoods) {
+                msg = "null argument";
+                return WHMEC_ERR_INPUT;
+            }
+            if (sg->continues && !alpha_in) {
+                msg = "genotyping segments: a segment that continues the table needs alpha_in (the forward vector in front of it)";
+                return WHMEC_ERR_INPUT;
+            }
+            if (sg->continued && !beta_in) {
+                msg = "genotyping segments: a segment that the table continues after needs beta_in (the backward vector behind it)";
+                return WHMEC_ERR_INPUT;
+            }
+            CUDA_TRY(cudaSetDevice(sg->device));
+            uint64_t budget = 0;  // the inputs are resident already: counted twice, which errs on the safe side
+            const int rc = work_budget(sg->pk, sg->g, budget, msg);
+            if (rc != WHMEC_OK) return rc;
+            return run_packed(sg->B, sg->pk, sg->g, sg->v, budget, sg->continues ? alpha_in : nullptr, sg->continued ? beta_in : nullptr, likelihoods, st,
+                              sg->h2d, msg);
+        },
+        err, errlen);
+}
+
+extern "C" void whmec_genotype_segment_destroy(whmec_gl_segment *sg) {
+    if (!sg) return;
+    cudaSetDevice(sg->device);
+    delete sg;
 }

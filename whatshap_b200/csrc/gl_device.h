@@ -127,4 +127,33 @@ WHMEC_HD void gl_forward_cell(const GlView &v, uint32_t k, uint32_t x, const dou
     }
 }
 
+// One cell of the transfer pass of a segment (gl_transfer_plan): the forward recursion of column k for n_in input rows at
+// once, without posterior and without backward tables.  prev / cur hold one row per input, [u][2^f * T] (the row stride of
+// column k is 2^f_k * T; before a segment's column 0, prev holds the inputs themselves, [u][T]).  The partition products and
+// the emission are computed once per (x, i) and reused for every input.  Unlike gl_forward_cell, the table's last column
+// adds its values too: the mass the segment leaves at every transmission value.
+template <class Add>
+WHMEC_HD void gl_transfer_cell(const GlView &v, uint32_t k, uint32_t x, uint32_t n_in, const double *prev, double *cur, Add add) {
+    const GlCol &c = v.cols[k];
+    const uint32_t T = v.T, nA = 1u << v.P;
+    const uint32_t o = pext32(x, c.keep), b = x & low_mask(c.bw);
+    const uint64_t out_w = ((uint64_t)1 << c.f) * T, in_w = k ? ((uint64_t)1 << v.cols[k - 1].f) * T : T;
+    const double *t = v.trans + c.trans_off;
+    double cp[GL_MAX_P][2];
+    for (uint32_t i = 0; i < T; ++i) {
+        gl_partition_products(v, c, x, i, cp);
+        double E = 0.0;
+        for (uint32_t A = 0; A < nA; ++A) E += gl_emission(cp, v.P, A) * v.q[c.q_off + (size_t)i * nA + A];
+        for (uint32_t u = 0; u < n_in; ++u) {
+            double S = 1.0;
+            if (!c.first) {
+                S = 0.0;
+                const double *p = prev + u * in_w + (size_t)b * T;
+                for (uint32_t j = 0; j < T; ++j) S += p[j] * t[(size_t)j * T + i];
+            }
+            add(&cur[u * out_w + (size_t)o * T + i], S * E);
+        }
+    }
+}
+
 }  // namespace whmec

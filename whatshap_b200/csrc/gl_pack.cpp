@@ -23,7 +23,26 @@ long double phred_probability(uint32_t phred) {  // genotypecolumncostcomputer.c
 
 }  // namespace
 
-int gl_pack(const whmec_problem *p, Packed &pk, GlPacked &g, std::string &err) {
+namespace {
+
+int pack_impl(const whmec_problem *p, bool continues, bool continued, Packed &pk, GlPacked &g, std::string &err);
+
+}  // namespace
+
+int gl_pack(const whmec_problem *p, Packed &pk, GlPacked &g, std::string &err) { return pack_impl(p, false, false, pk, g, err); }
+
+int gl_pack_segment(const whmec_problem *p, bool continues, bool continued, Packed &pk, GlPacked &g, std::string &err) {
+    int rc = pack_impl(p, continues, continued, pk, g, err);
+    if (rc == WHMEC_OK && pk.T == 1) {
+        err = "genotyping segments: a single individual's chains are independent tables already (shard them with whmec_genotype)";
+        return WHMEC_ERR_UNSUPPORTED;
+    }
+    return rc;
+}
+
+namespace {
+
+int pack_impl(const whmec_problem *p, bool continues, bool continued, Packed &pk, GlPacked &g, std::string &err) {
     g = GlPacked();
     if (p->n_cols > 0 && !p->gl) {
         // assert(gls != nullptr), transitionprobabilitycomputer.cpp:66
@@ -61,8 +80,8 @@ int gl_pack(const whmec_problem *p, Packed &pk, GlPacked &g, std::string &err) {
         // Without transmission values (T == 1) a chain boundary hands over a single number, which cancels in the
         // per-column normalisation: every DP-independent chain is then a table of its own (and they can be
         // processed group by group when the backward tables of all columns do not fit the device).
-        c.first = (k == 0) || (T == 1 && pk.cols[k - 1].f == 0);
-        c.last = (k + 1 == n) || (T == 1 && m.f == 0);
+        c.first = (k == 0 && !continues) || (k > 0 && T == 1 && pk.cols[k - 1].f == 0);
+        c.last = (k + 1 == n && !continued) || (T == 1 && m.f == 0);
         c.act_off = pk.act_off[k];
         c.beta_off = g.beta_doubles;
         const uint64_t proj = ((uint64_t)1 << m.f) * T;
@@ -108,10 +127,16 @@ int gl_pack(const whmec_problem *p, Packed &pk, GlPacked &g, std::string &err) {
     return WHMEC_OK;
 }
 
+// doubles of B_k: none for a table's last column; a continued segment's last column owns T (beta_in)
+uint64_t own_beta(const GlPacked &g, uint32_t T, uint32_t k) { return g.cols[k].last ? 0 : ((uint64_t)1 << g.cols[k].f) * T; }
+
+}  // namespace
+
 void gl_schedule(const GlPacked &g, uint32_t T, uint32_t lo, uint32_t hi, GlSchedule &out) {
     out = GlSchedule();
     out.beta_base = g.cols[lo].beta_off;
-    out.beta_doubles = g.cols[hi - 1].beta_off - out.beta_base;  // the group ends a table: its last column owns no entries
+    // the group ends a table: its last column owns no entries, unless the table is continued in another segment
+    out.beta_doubles = g.cols[hi - 1].beta_off + own_beta(g, T, hi - 1) - out.beta_base;
     struct Table {
         uint32_t begin, end;  // columns [begin, end)
         uint64_t f_off, f_size;
@@ -119,8 +144,8 @@ void gl_schedule(const GlPacked &g, uint32_t T, uint32_t lo, uint32_t hi, GlSche
     std::vector<Table> tables;
     uint32_t longest = 0;
     for (uint32_t k = lo, begin = lo; k < hi; ++k)
-        if (g.cols[k].last) {
-            uint64_t size = 1;
+        if (g.cols[k].last || k + 1 == hi) {
+            uint64_t size = g.cols[begin].first ? 1 : T;  // a continuing segment: F_{lo-1} = alpha_in, T entries
             for (uint32_t q = begin; q <= k; ++q)
                 if (!g.cols[q].last) size = std::max(size, ((uint64_t)1 << g.cols[q].f) * T);
             tables.push_back(Table{begin, k + 1, out.f_pool_doubles, size});
@@ -165,14 +190,14 @@ void gl_groups_split(const GlPacked &g, uint32_t T, uint64_t budget, std::vector
     begin.assign(1, 0);
     alone.clear();
     const uint32_t n = (uint32_t)g.cols.size();
-    uint64_t run = 0, table = 0, widest = 1;
+    uint64_t run = 0, table = 0, widest = (n && !g.cols[0].first) ? T : 1;  // a continuing segment: alpha_in in the F pool
     uint32_t table_begin = 0;
     for (uint32_t k = 0; k < n; ++k) {
         if (!g.cols[k].last) {
             const uint64_t proj = ((uint64_t)1 << g.cols[k].f) * T;
             table += proj;
             widest = std::max(widest, proj);
-            continue;
+            if (k + 1 < n) continue;  // a continued segment's table ends at its last column all the same
         }
         const uint64_t cost = table + 2 * widest;  // a table ends here: its backward tables and its two projection buffers
         if (cost > budget) {  // a group of its own: close the open group (if any) before it and start a new one after it
@@ -210,11 +235,12 @@ bool gl_groups(const GlPacked &g, uint32_t T, uint64_t budget, std::vector<uint3
 bool gl_bounded(const GlPacked &g, uint32_t T, uint32_t lo, uint32_t hi, uint64_t budget, GlBounded &out) {
     out = GlBounded();
     const uint32_t m = hi - lo;
-    auto own = [&](uint32_t k) { return g.cols[k].last ? 0 : ((uint64_t)1 << g.cols[k].f) * T; };  // doubles of B_k
-    uint64_t f_size = 1;
+    auto own = [&](uint32_t k) { return own_beta(g, T, k); };  // doubles of B_k
+    uint64_t f_size = g.cols[lo].first ? 1 : T;  // a continuing segment: F_{lo-1} = alpha_in, T entries
     for (uint32_t k = lo; k < hi; ++k) f_size = std::max(f_size, own(k));
     out.f_pool_doubles = 2 * f_size;
-    if (budget <= out.f_pool_doubles) return false;
+    const uint64_t tail = own(hi - 1);  // a continued segment: beta_in, the checkpoint of the last segment
+    if (budget <= out.f_pool_doubles + tail) return false;
     // mirrored order: column j is column hi - 1 - j.  A mirrored segment that starts at j + 1 is a segment that ends at column
     // hi - 2 - j; its checkpoint is B_{hi - 2 - j}.
     std::vector<uint64_t> off(m + 1, 0), ck(m, 0);
@@ -223,17 +249,19 @@ bool gl_bounded(const GlPacked &g, uint32_t T, uint32_t lo, uint32_t hi, uint64_
         if (j + 1 < m) ck[j] = own(hi - 2 - j);
     }
     std::vector<uint32_t> mcuts;
-    if (!cut_column_segments(off, ck, budget - out.f_pool_doubles, mcuts, out.arena_doubles, out.ckpt_doubles)) return false;
+    if (!cut_column_segments(off, ck, budget - out.f_pool_doubles - tail, mcuts, out.arena_doubles, out.ckpt_doubles)) return false;
+    out.ckpt_doubles += tail;
     for (size_t c = mcuts.size(); c-- > 0;) out.cuts.push_back(hi - mcuts[c]);
     const uint32_t S = (uint32_t)out.cuts.size() - 1;
     const std::vector<uint32_t> &c = out.cuts;
     const uint64_t A = out.arena_doubles;
-    std::vector<uint64_t> ckpt(S, 0);  // store offset of segment s's checkpoint (s < S - 1)
+    std::vector<uint64_t> ckpt(S, 0);  // store offset of segment s's checkpoint (s < S - 1; s = S - 1 only with a tail)
     uint64_t at = 0;
-    for (uint32_t s = 0; s + 1 < S; ++s) {
+    for (uint32_t s = 0; s + 1 < S || (tail && s < S); ++s) {
         ckpt[s] = A + at;
         at += own(c[s + 1] - 1);
     }
+    if (tail) out.tail_off = ckpt[S - 1];
     auto beta_off = [&](uint32_t k) { return g.cols[k].beta_off; };
     auto backward = [&](uint32_t k, uint64_t dst) {  // column k reads B_k, adds into B_{k-1} at dst
         GlStep st{};
@@ -248,7 +276,7 @@ bool gl_bounded(const GlPacked &g, uint32_t T, uint32_t lo, uint32_t hi, uint64_
         const uint64_t base = beta_off(c[s]);
         sw.beta_base = base;
         sw.clear = clear ? beta_off(c[s + 1] - 1) - base : 0;
-        if (s + 1 < S) {
+        if (s + 1 < S || tail) {
             sw.copy_dst = beta_off(c[s + 1] - 1) - base;
             sw.copy_src = ckpt[s];
             sw.copy_n = own(c[s + 1] - 1);
@@ -297,19 +325,26 @@ int gl_plan(const GlPacked &g, uint32_t T, uint64_t budget, std::vector<GlUnit> 
     for (size_t q = 0; q < units.size(); ++q) {
         GlUnit &u = units[q];
         u.bounded = alone[q];
+        const uint32_t hi = begin[q + 1];
         if (!u.bounded) {
-            gl_schedule(g, T, begin[q], begin[q + 1], u.sc);
+            gl_schedule(g, T, begin[q], hi, u.sc);
             u.work_doubles = u.sc.beta_doubles + 1 + u.sc.f_pool_doubles;
-        } else if (gl_bounded(g, T, begin[q], begin[q + 1], budget, u.bd)) {
-            u.work_doubles = u.bd.arena_doubles + u.bd.ckpt_doubles + u.bd.f_pool_doubles;
-        } else {  // the least budget with a cut that fits (bisection), at most the table's resident cost
+            u.alpha_at = u.sc.beta_doubles + 1 + u.sc.steps[u.sc.fwd_begin[0]].prev_off;
+            u.beta_at = g.cols[hi - 1].beta_off - u.sc.beta_base;
+        } else if (gl_bounded(g, T, begin[q], hi, budget, u.bd)) {
+            const uint64_t store = u.bd.arena_doubles + u.bd.ckpt_doubles;
+            u.work_doubles = store + u.bd.f_pool_doubles;
+            u.alpha_at = store + u.bd.steps[u.bd.sweeps[u.bd.cuts.size() - 1].fwd_begin].prev_off;  // pass B's first step
+            u.beta_at = u.bd.tail_off;
+        } else {  // the least budget with a cut that fits (bisection), at most the table's resident cost.  A continued segment keeps
+                  // beta_in twice there: in its last column's backward table (beta_doubles) and as the last segment's checkpoint
             GlSchedule whole;
-            gl_schedule(g, T, begin[q], begin[q + 1], whole);
-            uint64_t no = budget, yes = whole.beta_doubles + whole.f_pool_doubles;
+            gl_schedule(g, T, begin[q], hi, whole);
+            uint64_t no = budget, yes = whole.beta_doubles + whole.f_pool_doubles + own_beta(g, T, hi - 1);
             GlBounded probe;
             while (yes - no > 1) {
                 const uint64_t mid = no + (yes - no) / 2;
-                (gl_bounded(g, T, begin[q], begin[q + 1], mid, probe) ? yes : no) = mid;
+                (gl_bounded(g, T, begin[q], hi, mid, probe) ? yes : no) = mid;
             }
             need = std::max(need, yes);
         }
@@ -320,6 +355,55 @@ int gl_plan(const GlPacked &g, uint32_t T, uint64_t budget, std::vector<GlUnit> 
         return WHMEC_ERR_UNSUPPORTED;
     }
     return WHMEC_OK;
+}
+
+void gl_transfer_plan(const GlPacked &g, uint32_t T, bool continues, GlTransfer &out) {
+    out = GlTransfer();
+    const uint32_t n = (uint32_t)g.cols.size();
+    out.n_in = continues ? std::min(T, GL_T_LOCAL) : 1;
+    out.n_batches = continues ? T / out.n_in : 1;
+    uint64_t f_size = T;  // the inputs: [u][T]
+    for (uint32_t k = 0; k < n; ++k) f_size = std::max(f_size, ((uint64_t)1 << g.cols[k].f) * T);
+    const uint64_t half = f_size * out.n_in;
+    out.f_pool_doubles = 2 * half;
+    for (uint32_t k = 0; k < n; ++k) {
+        GlStep st{};
+        st.k = k;
+        st.cells_log2 = g.cols[k].a;
+        st.cur_off = (uint64_t)(k & 1) * half;
+        st.prev_off = (uint64_t)((k + 1) & 1) * half;
+        st.n_scale = ((uint64_t)1 << g.cols[k].f) * T * out.n_in;
+        st.n_clear = half;
+        out.steps.push_back(st);
+    }
+    out.in_off = half;                       // steps[0].prev_off
+    out.out_off = n ? out.steps[n - 1].cur_off : 0;
+}
+
+void gl_transfer_combine(const GlTransfer &tp, uint32_t T, const std::vector<double> &rows, const std::vector<double> &col_max, double *m) {
+    if (tp.n_in * tp.n_batches < T) {  // a segment that starts the table: every row is the one row it computed
+        for (uint32_t u = 0; u < T; ++u) std::copy(rows.begin(), rows.begin() + T, m + (size_t)u * T);
+        return;
+    }
+    const size_t n = tp.steps.size(), B = tp.n_batches;
+    std::vector<long double> mant(B, 1.0L);  // batch b's product of scales = mant[b] * 2^ex[b], mant in [0.5, 1)
+    std::vector<int64_t> ex(B, 0);
+    for (size_t b = 0; B > 1 && b < B; ++b)
+        for (size_t k = 0; k < n; ++k) {
+            const double mx = col_max[b * n + k];
+            if (!(mx > 0.0)) continue;  // an all-zero column is not divided (its rows stay 0)
+            int e = 0;
+            mant[b] = frexpl(mant[b] * (long double)mx, &e);
+            ex[b] += e;
+        }
+    size_t top = 0;
+    for (size_t b = 1; b < B; ++b)
+        if (ex[b] > ex[top] || (ex[b] == ex[top] && mant[b] > mant[top])) top = b;
+    for (size_t b = 0; b < B; ++b) {
+        const int64_t d = std::max<int64_t>(ex[b] - ex[top], -100000);  // far below the smallest double: 0
+        const double f = B > 1 ? (double)ldexpl(mant[b] / mant[top], (int)d) : 1.0;
+        for (size_t e = b * tp.n_in * T; e < (b + 1) * tp.n_in * T; ++e) m[e] = rows[e] * f;
+    }
 }
 
 void gl_scale_host(double *v, uint64_t n) {

@@ -8,7 +8,9 @@ no collective on the data path, and the per-block results are gathered on rank 0
 couple the blocks through the transmission vector: every rank holds a SEGMENT of the table
 (`whmec_segment_*`) and the ranks exchange T x T transfer matrices and exit tables (two all-gathers of a
 few hundred bytes), bit-identical to the single-GPU solve.  `genotype_sharded` does the same by chains for the
-forward-backward genotyping DP of a single individual.
+forward-backward genotyping DP of a single individual, and by segments of the table for a pedigree: every rank holds a
+segment (`whmec_genotype_segment_*`), the ranks all-gather T x T transfer matrices of doubles, fold them into every
+segment's true forward and backward inputs, and each runs its segment (DESIGN §4.5).
 
 The reference has no counterpart (single process, `whatshap/cli/phase.py:604-610` runs one
 PedigreeDPTable per chromosome x family).
@@ -384,15 +386,80 @@ def solve_sharded(prob: Optional[FlatProblem], solver: Optional[Callable[[FlatPr
     return out
 
 
+def _scaled(vec: np.ndarray) -> np.ndarray:
+    """`vec` divided by its largest entry; unchanged when every entry is 0 (gl_scale_host)."""
+    top = float(vec.max()) if vec.size else 0.0
+    return vec / top if top > 0.0 else vec
+
+
+def genotype_segment_inputs(matrices: Sequence[Optional[np.ndarray]]) -> Tuple[List[Optional[np.ndarray]], List[Optional[np.ndarray]]]:
+    """True forward input (alpha) and backward input (beta) of every genotyping segment from the segments' T x T transfer
+    matrices (None: rank without columns; it gets None for both).  The first segment ignores its input: any row of its
+    matrix is its output.  The last segment's matrix holds the mass it leaves at every transmission value, so its row sums
+    are the backward vector in front of it.  Left to right alpha_{s+1} = alpha_s . M_s, right to left beta_s = M_{s+1} .
+    beta_{s+1}; every vector is divided by its largest entry (a positive factor cancels in the per-column normalisation).
+    alpha is None for the first segment, beta for the last."""
+    active = [s for s, m in enumerate(matrices) if m is not None]
+    alphas: List[Optional[np.ndarray]] = [None] * len(matrices)
+    betas: List[Optional[np.ndarray]] = [None] * len(matrices)
+    vec = None
+    for s in active:
+        alphas[s] = vec
+        m = np.asarray(matrices[s], np.float64)
+        vec = _scaled(m[0].copy() if vec is None else vec @ m)
+    vec = None
+    for s in reversed(active):
+        betas[s] = vec
+        m = np.asarray(matrices[s], np.float64)
+        vec = _scaled(m @ (np.ones(m.shape[1]) if vec is None else vec))
+    return alphas, betas
+
+
+def _default_genotype_segment_factory():
+    import torch
+
+    from . import _lib
+
+    device = torch.cuda.current_device()
+    return lambda p, continues, continued: _lib.GenotypeSegment(p, continues, continued, device=device)
+
+
+def genotype_pedigree_segments(prob: FlatProblem, n_segments: int, segment_factory=None) -> np.ndarray:
+    """The multi-GPU pedigree genotyping scheme with all `n_segments` segments driven by ONE process on one device, in the
+    order the ranks would run them: transfer matrices, the fold, then every segment's run.  Returns [n_ind, n_cols, 3]."""
+    if segment_factory is None:
+        segment_factory = _default_genotype_segment_factory()
+    ranges = segment_ranges(prob, n_segments)
+    out = np.zeros((prob.n_ind, prob.n_cols, 3), np.float64)
+    segs = []
+    try:
+        for r in ranges:
+            segs.append(None if r is None else segment_factory(prob.slice_columns(*r), r[0] > 0, r[1] < prob.n_cols))
+        alphas, betas = genotype_segment_inputs([sg.transfer() if sg else None for sg in segs])
+        for r, sg, a, b in zip(ranges, segs, alphas, betas):
+            if sg:
+                out[:, r[0]:r[1], :] = sg.run(a, b)
+    finally:
+        for sg in segs:
+            if sg:
+                sg.close()
+    return out
+
+
 def genotype_sharded(prob: Optional[FlatProblem], solver: Optional[Callable[[FlatProblem], np.ndarray]] = None,
-                     group=None, comm=None) -> Optional[np.ndarray]:
+                     group=None, comm=None, segment_factory=None) -> Optional[np.ndarray]:
     """Genotype likelihoods (`whmec_genotype`, the reference's GenotypeDPTable) of `prob` (given on rank 0; other ranks
     pass None) on all ranks of `group`; returns [n_ind, n_cols, 3] on rank 0, None elsewhere.
 
     Without transmission values every DP-independent chain is a forward-backward table of its own (a chain boundary hands
     over one number, which cancels in each column's normalisation), so a single individual shards like the phasing DP:
     every rank takes a contiguous run of whole chains balanced by DP cells, no collective on the data path, likelihoods
-    gathered on rank 0.  A pedigree is one table and runs on one GPU (replicas only).  Errors are raised on every rank."""
+    gathered on rank 0.  A pedigree with two chains or more is cut into segments of whole chains (`segment_ranges`), one
+    per rank: one all-gather of the T x T transfer matrices, the fold (`genotype_segment_inputs`), every rank runs its
+    segment, likelihoods gathered on rank 0.  A pedigree of one chain runs on rank 0's GPU, as does the whole table when
+    any rank's segment is refused as unsupported in any phase.  A refusal of the table on one GPU is raised as Unsupported on
+    every rank.  `solver` / `segment_factory` default to the CUDA path on this rank's
+    current device.  Errors are raised on every rank."""
     from . import _wire
 
     if solver is None:
@@ -406,26 +473,41 @@ def genotype_sharded(prob: Optional[FlatProblem], solver: Optional[Callable[[Fla
     rank, world = comm.rank, comm.world
     rows = None
     if rank == 0:
-        if prob.n_trios > 0 or prob.n_cols == 0 or world == 1:
-            rows = [_wire.join([np.array([0, 0, 0], np.int64).view(np.uint8)])] * world
+        blocks = independent_blocks(prob) if prob.n_cols and world > 1 else []
+        if prob.n_trios > 0 and len(blocks) > 1:  # transmission vectors couple the chains: segments of the table
+            rows = []
+            for r in segment_ranges(prob, world):
+                lo, hi = r if r is not None else (0, 0)
+                rows.append(_wire.join([np.array([2, lo, hi, prob.n_cols], np.int64).view(np.uint8)] +
+                                       ([_wire.encode_problem(prob.slice_columns(lo, hi), lo=lo)] if hi > lo else [])))
+        elif prob.n_trios > 0 or prob.n_cols == 0 or world == 1:
+            rows = [_wire.join([np.array([0, 0, 0, 0], np.int64).view(np.uint8)])] * world
         else:  # every rank receives only its run of chains
-            blocks = independent_blocks(prob)
             rows = []
             for b0, b1 in contiguous_shares(block_work(prob, blocks), world):
                 lo, hi = (blocks[b0][0], blocks[b1 - 1][1]) if b1 > b0 else (0, 0)
-                rows.append(_wire.join([np.array([1, lo, hi], np.int64).view(np.uint8)] +
+                rows.append(_wire.join([np.array([1, lo, hi, prob.n_cols], np.int64).view(np.uint8)] +
                                        ([_wire.encode_problem(prob.slice_columns(lo, hi), lo=lo)] if hi > lo else [])))
     pieces = _wire.separate(comm.scatter_rows(rows))
-    mode, lo, hi = (int(x) for x in pieces[0].view(np.int64))
+    mode, lo, hi, n_cols = (int(x) for x in pieces[0].view(np.int64))
     out, err = None, None
+    if mode == 2:
+        handled, out = _genotype_segment_rank(pieces[1] if len(pieces) > 1 else None, lo, hi, n_cols, comm, segment_factory)
+        if not handled:
+            mode = 0
     try:
         if mode == 0:
             out = solver(prob) if rank == 0 else None
-        elif len(pieces) > 1:
+        elif mode == 1 and len(pieces) > 1:
             out = np.ascontiguousarray(solver(_wire.decode_problem(pieces[1])[0]), np.float64)
     except Exception as e:  # noqa: BLE001
         err = e
-    _wire.raise_first_error(comm.all_status(*_wire.status_of(err)), "genotype")
+    if mode != 2:
+        states = comm.all_status(*_wire.status_of(err))
+        if _wire.raise_first_error(states, "genotype"):  # refused as unsupported: raised on every rank, as the one-GPU call raises it
+            from ._abi import Unsupported
+
+            raise Unsupported(next(text for kind, text, _ in states if kind == 1))
     if mode == 0:
         return out
     head = np.array([lo, hi], np.int64).view(np.uint8)
@@ -439,3 +521,46 @@ def genotype_sharded(prob: Optional[FlatProblem], solver: Optional[Callable[[Fla
             lo, hi = (int(x) for x in parts[0].view(np.int64))
             full[:, lo:hi, :] = parts[1].view(np.float64).reshape(prob.n_ind, hi - lo, 3)
     return full
+
+
+def _genotype_segment_rank(row: Optional[np.ndarray], lo: int, hi: int, n_cols: int, comm, segment_factory=None
+                           ) -> Tuple[bool, Optional[np.ndarray]]:
+    """This rank's part of `genotype_sharded` for a pedigree cut into segments: `row` holds its columns [lo, hi) of the
+    n_cols (None: no columns).  Returns (True, its likelihoods or None), or (False, None) on every rank when some rank
+    reports 'unsupported' in any phase (the caller then genotypes the whole table on rank 0's GPU, which gives what the
+    single-GPU call gives, its refusal included).  Every phase reports its status in the all-gather that follows
+    it, so an error on one rank is raised on every rank."""
+    from . import _wire
+
+    if segment_factory is None:
+        segment_factory = _default_genotype_segment_factory()
+    my_slice = _wire.decode_problem(row)[0] if row is not None else None
+    T = 1 << (2 * (my_slice.n_trios if my_slice is not None else 0))
+    seg = None
+
+    def phase(fn):
+        try:
+            return (0, ""), fn()
+        except Exception as e:  # noqa: BLE001 - reported to every rank below
+            return _wire.status_of(e), None
+
+    try:
+        status, seg = phase(lambda: segment_factory(my_slice, lo > 0, hi < n_cols) if my_slice is not None else None)
+        if _wire.raise_first_error(comm.all_status(*status), "create"):
+            return False, None
+        status, matrix = phase(lambda: seg.transfer() if seg else None)
+        T_all = max(comm.lengths(T))  # ranks without columns do not know T
+        states = comm.all_status(*status, payload=None if matrix is None else np.ascontiguousarray(matrix, np.float64),
+                                 payload_width=8 * T_all * T_all)
+        if _wire.raise_first_error(states, "transfer"):
+            return False, None
+        matrices = [None if pl is None else pl.view(np.float64).reshape(T_all, T_all).copy() for _, _, pl in states]
+        alphas, betas = genotype_segment_inputs(matrices)
+        status, out = phase(lambda: np.ascontiguousarray(seg.run(alphas[comm.rank], betas[comm.rank]), np.float64) if seg else None)
+        # e.g. a segment whose backward tables find no room on its device: no rank may return a partial table
+        if _wire.raise_first_error(comm.all_status(*status), "run"):
+            return False, None
+    finally:
+        if seg is not None:
+            seg.close()
+    return True, out
