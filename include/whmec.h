@@ -41,7 +41,8 @@ extern "C" {
 #define WHMEC_ERR_MENDELIAN 1   /* "Error: Mendelian conflict"   (pedigreedptable.cpp:301-303) */
 #define WHMEC_ERR_INPUT 2       /* unsorted reads / malformed arrays (columniterator.cpp:29,32) */
 #define WHMEC_ERR_CUDA 3        /* CUDA runtime failure, message in err */
-#define WHMEC_ERR_UNSUPPORTED 4 /* > 32 active reads (graycodes.cpp:12), cost range, a column beyond the HBM budget */
+#define WHMEC_ERR_UNSUPPORTED 4 /* > 32 active reads (graycodes.cpp:12), more than 5 trios (T > 1024), cost range, a column beyond the HBM
+                                   budget; five-trio tables: cost functions beyond 16 GiB, genotyping and table segments */
 
 /* allele codes in ent_allele (src/entry.h:8) */
 #define WHMEC_ALLELE_REF 0
@@ -102,7 +103,8 @@ typedef struct whmec_stats {
     float sweep_ms;              /* device time of the last forward sweep (CUDA events) */
     float h2d_ms, d2h_ms;        /* device-timed copies of the last solve */
     uint64_t h2d_bytes, d2h_bytes;
-    uint32_t path_kind;          /* 1 = tile kernel, 2 = column kernel, 3 = batched pedigree sweep, 4 = genotyping (forward-backward) */
+    uint32_t path_kind;          /* 1 = tile kernel, 2 = column kernel, 3 = batched pedigree sweep, 4 = genotyping (forward-backward),
+                                    5 = wide column sweep (five trios, T = 1024) */
     uint32_t reserved;
 } whmec_stats;
 
@@ -155,7 +157,7 @@ int whmec_genotype(const whmec_problem *p, double *likelihoods, int device, whme
  * if the probability of the others is < 0.1, else -1 (the reference's empty Genotype). */
 int whmec_compute_genotypes(const whmec_problem *p, double *gl, int8_t *gt, char *err, size_t errlen);
 
-/* ---- A pedigree table (T = 4^trios > 1) shared by several GPUs --------------------------------
+/* ---- A pedigree table (1 < T = 4^trios <= 256) shared by several GPUs --------------------------------
  * The reference sweeps a family's table on one thread (src/pedigreedptable.cpp:84-174).  Columns that no
  * read spans cut it into chains that exchange only the T projection values of the cut
  * (pedigreedptable.cpp:272-297), and a chain is min-plus linear in them.  A SEGMENT is a run of whole
@@ -176,7 +178,7 @@ int whmec_compute_genotypes(const whmec_problem *p, double *gl, int8_t *gt, char
  *   7. whmec_segment_finish   backtrace from `entry` (< 0: this segment ends the table) + outputs for the
  *                             segment's columns and reads; s->cost is the table's optimum iff entry < 0
  * Results are bit-identical to whmec_solve on the whole table.  WHMEC_ERR_UNSUPPORTED: single-individual
- * problems (their chains are independent, shard them with whmec_solve), costs beyond 2^28. */
+ * problems (their chains are independent, shard them with whmec_solve), costs beyond 2^28, five-trio tables (T = 1024). */
 int whmec_segment_create(const whmec_problem *p, int device, int continues, whmec_plan **out, char *err, size_t errlen);
 int whmec_segment_transfer(whmec_plan *plan, uint32_t *matrix /* [T*T] */, char *err, size_t errlen);
 int whmec_segment_sweep(whmec_plan *plan, const uint32_t *in_vec /* [T] or NULL */, uint32_t *out_vec /* [T] */,

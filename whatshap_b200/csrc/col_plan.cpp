@@ -71,7 +71,8 @@ int col_plan(Packed &pk, const ColPlanInput &in, ColPlan &plan, std::string &msg
     const uint32_t n = pk.n, T = pk.T, C = (uint32_t)pk.chain_begin.size() - 1;
     for (const ColMeta &m : pk.cols) plan.max_ent = std::max<uint64_t>(plan.max_ent, ((uint64_t)1 << m.f) * T);
     const uint64_t max_ent = plan.max_ent, free_b = in.free_bytes, hook = in.hook;
-    const uint64_t need = pk.bp_words * 4 + max_ent * (4 * 2 + 8) + pk.fn_delta.size() * 4 + (uint64_t)n * sizeof(ColMeta);
+    const bool wide = T > MAX_T;  // five trios: only the wide column sweep, which also holds the transformed projection (4 + 2 bytes)
+    const uint64_t need = pk.bp_words * 4 + max_ent * (4 * 2 + 8 + (wide ? 6 : 0)) + pk.fn_delta.size() * 4 + (uint64_t)n * sizeof(ColMeta);
     const uint64_t fixed = need - pk.bp_words * 4;  // everything but the back-pointers
     plan.fixed_bytes = fixed;
     const uint64_t hbm_budget = free_b > fixed + RESERVE ? free_b - fixed - RESERVE : 0;
@@ -86,7 +87,7 @@ int col_plan(Packed &pk, const ColPlanInput &in, ColPlan &plan, std::string &msg
         return WHMEC_ERR_UNSUPPORTED;
     }
     // which sweep: pedigrees with several chains take a two-pass sweep (fused trio kernel or batched), the rest the column sweep
-    const bool two_pass_shape = (C >= 2 || in.segment) && pk.safe31 && !(in.sequential && !in.segment);
+    const bool two_pass_shape = !wide && (C >= 2 || in.segment) && pk.safe31 && !(in.sequential && !in.segment);
     // one trio, shapes of ped_fused.h: one block per chain with the projection in shared memory (3 launches)
     bool fused = in.fused && T == PF_T && two_pass_shape;
     for (uint32_t k = 0; k < n && fused; ++k) fused = pf_column_ok(pk.cols[k], pk.fn_group.data() + pk.cols[k].grp_off);
@@ -171,7 +172,8 @@ int col_plan(Packed &pk, const ColPlanInput &in, ColPlan &plan, std::string &msg
             for (size_t sg = 0; sg < S; ++sg) add_steps(pk, plan, 1, plan.seg_chain[sg], plan.seg_chain[sg + 1], plan.seg_begin[sg], plan.seg_grid[sg]);
         }
     }
-    if (in.segment && plan.path == ColPath::column) {
+    if (wide) plan.path = ColPath::wide;
+    if (in.segment && !plan.two_pass()) {
         msg = "unsupported: this segment cannot run the two-pass pedigree sweep (costs beyond 2^28 or state beyond the budget)";
         return WHMEC_ERR_UNSUPPORTED;
     }

@@ -46,10 +46,10 @@ struct ColPlanInput {
     uint32_t cluster = 0;        // WHMEC_PED_CLUSTER: 1, 2, 4 or 8 forces the fused sweep's cluster size; anything else: automatic
 };
 
-enum class ColPath { column, batched, fused };
+enum class ColPath { column, batched, fused, wide };  // wide: the column sweep of T = 1024 (DESIGN §4.7)
 
 struct ColPlan {
-    ColPath path = ColPath::column;  // batched and fused are the two-pass sweeps
+    ColPath path = ColPath::column;  // batched and fused are the two-pass sweeps, wide sweeps column by column as `column`
     uint64_t max_ent = 1;            // largest column (entries): the size of each value buffer
     uint64_t slots = 0;              // batched sweep: value-buffer slots, (chain, unit vector) instances + one per chain
     uint64_t fixed_bytes = 0;        // device memory of the plan besides the back-pointers and the batch buffers
@@ -69,7 +69,7 @@ struct ColPlan {
     std::vector<uint32_t> ped_begin[3], ped_grid[3];  // [0] pass 1 (per-input instances), [1] pass 2, [2] pass 1 multi-RHS
     std::vector<std::vector<uint32_t>> seg_begin, seg_grid;  // bounded: pass 2 of every segment (instead of ped_begin[1])
     uint32_t cluster = 1;            // fused sweep: CTAs per chain
-    bool two_pass() const { return path != ColPath::column; }
+    bool two_pass() const { return path == ColPath::batched || path == ColPath::fused; }
 };
 
 // Plans the column-kernel sweep of `pk` (packed with deltas) and rebases pk.cols[k].bp_off when the plan is bounded.

@@ -17,7 +17,9 @@ namespace whmec {
 
 constexpr uint32_t UMAX = 0xFFFFFFFFu;  // +infinity of the reference's unsigned arithmetic
 constexpr uint32_t MAX_ACTIVE = 32;     // the reference's limit (graycodes.cpp:12, columnindexingscheme.cpp:42-44): a cell index is 32 bits
-constexpr uint32_t MAX_T = 256;         // 4 trios
+constexpr uint32_t MAX_T = 256;         // 4 trios: every path but the wide column sweep (DESIGN §4.7)
+constexpr uint32_t WIDE_T = 1024;       // 5 trios: the wide column sweep only
+constexpr uint64_t WIDE_FN_BYTES_MAX = 16ull << 30;  // host and device bytes of the cost functions a five-trio table may use
 constexpr uint32_t FN_STRIDE = 32;      // deltas per cost function
 
 // One variant column.  Bit j of a bipartition index <-> j-th active read (ascending read index).

@@ -40,7 +40,10 @@ struct ColView {
     // with prevarg the smallest minimising j (transition_min below).  Exact whenever no 32-bit sum
     // wraps (the batched pedigree path requires that); nullptr: raw values in `prev`.
     const uint32_t *prevm;
-    const uint8_t *prevarg;
+    union {
+        const uint8_t *prevarg;     // T <= 256
+        const uint16_t *prevarg16;  // T = 1024 (eval_candidates<true>, the wide column sweep)
+    };
 };
 
 // min over the previous transmission value for target value i (pedigreedptable.cpp:270-297 without the
@@ -83,7 +86,7 @@ WHMEC_HD void build_cost_table_run(const int32_t *delta /* [FN_STRIDE] of F */, 
 // Best key over candidates r in [r0, r1) of forward-projection entry `o` for transmission value i.
 // Reference: one iteration of the Gray-code loop body (pedigreedptable.cpp:239-327), restricted
 // to the candidates projecting onto `o` and visited in the same relative order.
-template <int NFR, bool EXACT = false>
+template <int NFR, bool EXACT = false, bool WIDE = false>
 WHMEC_HD uint64_t eval_candidates_t(const ColView &v, uint32_t o, uint32_t i, uint32_t r0, uint32_t r1) {
     const ColMeta &m = *v.m;
     const uint32_t drop = ~m.keep & low_mask(m.a);
@@ -175,7 +178,10 @@ WHMEC_HD uint64_t eval_candidates_t(const ColView &v, uint32_t o, uint32_t i, ui
         }
     }
     // the argmin j of the winner is looked up once (it never decides between candidates: r is unique)
-    if (v.prevm && !m.first && (uint32_t)(best >> 32) != UMAX) best |= v.prevarg[(size_t)best_b * v.T + i];
+    if (v.prevm && !m.first && (uint32_t)(best >> 32) != UMAX) {
+        if constexpr (WIDE) best |= v.prevarg16[(size_t)best_b * v.T + i];
+        else best |= v.prevarg[(size_t)best_b * v.T + i];
+    }
     return best;
 }
 
@@ -237,16 +243,18 @@ WHMEC_HD void eval_values_multi(const ColView &v, uint32_t o, uint32_t i, uint32
 }
 
 // Dispatch on the number of cost functions of the transmission group: the common small groups get a
-// small code path (the whole kernel otherwise thrashes the instruction cache).
+// small code path (the whole kernel otherwise thrashes the instruction cache).  WIDE: the argmins of
+// the transformed projection are 16-bit (T = 1024).
+template <bool WIDE = false>
 WHMEC_HD uint64_t eval_candidates(const ColView &v, uint32_t o, uint32_t i, uint32_t r0, uint32_t r1) {
     switch (v.nf) {  // exact small counts: no per-function predicates in the candidate loop
-        case 1: return eval_candidates_t<1, true>(v, o, i, r0, r1);
-        case 2: return eval_candidates_t<2, true>(v, o, i, r0, r1);
-        case 3: return eval_candidates_t<3, true>(v, o, i, r0, r1);
-        case 4: return eval_candidates_t<4, true>(v, o, i, r0, r1);
+        case 1: return eval_candidates_t<1, true, WIDE>(v, o, i, r0, r1);
+        case 2: return eval_candidates_t<2, true, WIDE>(v, o, i, r0, r1);
+        case 3: return eval_candidates_t<3, true, WIDE>(v, o, i, r0, r1);
+        case 4: return eval_candidates_t<4, true, WIDE>(v, o, i, r0, r1);
         default: break;
     }
-    return eval_candidates_t<NF_REG>(v, o, i, r0, r1);
+    return eval_candidates_t<NF_REG, false, WIDE>(v, o, i, r0, r1);
 }
 
 // One backtrace step (pedigreedptable.cpp:155-160): given the back-pointer word of entry

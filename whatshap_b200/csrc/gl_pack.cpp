@@ -49,6 +49,10 @@ int pack_impl(const whmec_problem *p, bool continues, bool continued, Packed &pk
         err = "genotyping needs genotype likelihoods (priors) for every individual and column";
         return WHMEC_ERR_INPUT;
     }
+    if (p->n_trios > 4 && p->n_trios < p->n_ind) {  // (before packing: with every assignment allowed, T = 1024 packs 2^20 functions per column)
+        err = "unsupported: genotyping supports at most 4 trio relationships (T = 4^trios <= 256)";
+        return WHMEC_ERR_UNSUPPORTED;
+    }
     whmec_problem q = *p;
     q.distrust = 1;  // the column structure does not depend on genotypes; no genotype constraint applies here
     int rc = pack_problem(&q, pk, err, false);

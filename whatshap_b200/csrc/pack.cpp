@@ -86,9 +86,9 @@ int pack_problem(const whmec_problem *p, Packed &pk, std::string &err, bool want
         err = "pedigree must have between 1 and 16 individuals";
         return WHMEC_ERR_UNSUPPORTED;
     }
-    if (p->n_trios >= p->n_ind || p->n_trios > 4) {
-        err = "unsupported pedigree: at most 4 trio relationships (T = 4^trios <= 256)";
-        return p->n_trios > 4 ? WHMEC_ERR_UNSUPPORTED : WHMEC_ERR_INPUT;
+    if (p->n_trios >= p->n_ind || p->n_trios > 5) {
+        err = "unsupported pedigree: at most 5 trio relationships (T = 4^trios <= 1024)";
+        return p->n_trios > 5 ? WHMEC_ERR_UNSUPPORTED : WHMEC_ERR_INPUT;
     }
     pk.P = 2 * (p->n_ind - p->n_trios);
     if (pk.P > MAX_P) {
@@ -286,6 +286,16 @@ int pack_problem(const whmec_problem *p, Packed &pk, std::string &err, bool want
                 fn_off_of[k + 1] = count;  // 0: Mendelian conflict, reported by the chunk worker in column order
             }
         });
+        // one function per (transmission value, allowed assignment): with T = 1024 and distrusted genotypes a column can hold 2^20
+        // of them (147 MB), so five-trio inputs are refused before the arrays are allocated
+        uint64_t fn_count = 0;
+        for (uint32_t k = 0; k < n; ++k) fn_count += fn_off_of[k + 1];
+        const uint64_t fn_bytes = fn_count * (3 * 4 + (want_deltas ? FN_STRIDE * 4 : 0));
+        if (T > MAX_T && fn_bytes > WIDE_FN_BYTES_MAX) {
+            err = "unsupported: the cost functions of this five-trio pedigree need " + std::to_string(fn_bytes) + " bytes (at most " +
+                  std::to_string(WIDE_FN_BYTES_MAX) + ")";
+            return WHMEC_ERR_UNSUPPORTED;
+        }
         for (uint32_t k = 0; k < n; ++k) fn_off_of[k + 1] += fn_off_of[k];
         const size_t fn_total = fn_off_of[n];
         pk.fn_c0.resize(fn_total);
@@ -454,6 +464,7 @@ int pack_problem(const whmec_problem *p, Packed &pk, std::string &err, bool want
     }
     pk.act_off[n] = pk.act_read.size();
     pk.safe31 = (phred_total + base_total + rc_total) < (1ull << 28);
+    pk.nowrap = (phred_total + base_total + rc_total) < UMAX;
     const auto t_merge = tnow();
     if (timing)
         std::fprintf(stderr, "[whmec] pack: validate %.2f ms, count + chunks(%u) %.2f ms, totals %.2f ms\n", tms(t_start, t_valid), n_chunks,

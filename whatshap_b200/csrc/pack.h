@@ -15,6 +15,8 @@ struct Packed {
     uint32_t T = 1, tb = 0, P = 2;
     bool has_deltas = true;              // fn_delta filled
     bool safe31 = false;                 // every reachable cost value < 2^30 (tile-kernel arithmetic is exact)
+    bool nowrap = false;                 // every reachable value plus a column's transition cost < 2^32 - 1: no 32-bit sum wraps
+                                         // (the wide path's transition transform is exact, DESIGN §4.7)
     // (RawVec: resize() does not zero-fill; every element is written by the packer)
     StagedVec<ColMeta> cols;             // [n]  (uploaded as it is: page-locked when the CUDA side installed its pool)
     // active reads per column, CSR aligned with cols[k].a

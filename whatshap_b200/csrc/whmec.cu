@@ -31,6 +31,7 @@
 #include "grouped.h"
 #include "pack.h"
 #include "tile.cuh"
+#include "wide_device.h"
 
 using namespace whmec;
 
@@ -760,6 +761,72 @@ __global__ void __launch_bounds__(256) col_finalize_kernel(const ColMeta *__rest
     bp_store_warp(arena, m.bp_off, m.bp_width, e, bpv, e < nent);
 }
 
+// ------------------------------------------------------------------------------------------
+// Wide column sweep (T = 1024, five trios; DESIGN §4.7).  Two kernels per column: the transition transform of the previous
+// projection (T^2 -> T log2 T per projection index), then the column step into one key per entry, which col_finalize_kernel
+// turns into values and back-pointers.  The per-thread code is in wide_device.h.
+// ------------------------------------------------------------------------------------------
+
+// One block per backward-projection index b: prevm[b][i] = min_j(prev[b][j] + popcount(i ^ j) * rc) with the smallest minimising j.
+// Bits 0..4 of i ^ j are relaxed across the lanes of a warp, bits 5..9 through shared memory.  prev == nullptr: the table's
+// first column, whose previous values are all 0.
+__global__ void __launch_bounds__(WIDE_T) wide_xform_kernel(const uint32_t *__restrict__ prev, uint32_t rc, uint32_t *__restrict__ prevm,
+                                                            uint16_t *__restrict__ prevarg) {
+    __shared__ unsigned long long keys[WIDE_T];
+    const uint32_t i = threadIdx.x;
+    const uint64_t row = (uint64_t)blockIdx.x * WIDE_T;
+    uint64_t key = wide_key(prev ? prev[row + i] : 0u, i);
+    for (uint32_t q = 0; q < 5; ++q) key = wide_relax(key, __shfl_xor_sync(0xFFFFFFFFu, key, 1u << q), rc);
+    for (uint32_t q = 5; q < WIDE_TB; ++q) {
+        keys[i] = key;
+        __syncthreads();
+        key = wide_relax(key, keys[i ^ (1u << q)], rc);
+        __syncthreads();
+    }
+    prevm[row + i] = wide_key_value(key);
+    prevarg[row + i] = wide_key_arg(key);
+}
+
+// Thread gid owns candidate chunk c = gid mod 2^L of entry e = gid >> L (wide_chunk_bits).  The group table is read from global
+// memory.  L <= 5: the chunks of an entry meet in a warp reduction and the entry's key is stored; L > 5: warps meet in a 64-bit
+// atomicMin on keys (preset to KEY_INF).  prevm == nullptr: raw previous values (a sum may wrap, Packed::nowrap), the O(T) loop.
+// With prevm, cm.first is 0 even for the table's first column: its transform ran on zeros.
+__global__ void __launch_bounds__(256) wide_step_kernel(const __grid_constant__ ColMeta cm, const uint32_t *__restrict__ fn_c0,
+                                                        const int32_t *__restrict__ fn_delta, const uint32_t *__restrict__ fn_group,
+                                                        const uint32_t *__restrict__ prev, const uint32_t *__restrict__ prevm,
+                                                        const uint16_t *__restrict__ prevarg, uint32_t L, unsigned long long *__restrict__ keys) {
+    const uint64_t nent = ((uint64_t)1 << cm.f) * WIDE_T;
+    const uint64_t gid = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const uint64_t e = gid >> L;
+    unsigned long long key = KEY_INF;
+    if (e < nent) {
+        const uint32_t o = (uint32_t)(e >> WIDE_TB), i = (uint32_t)e & (WIDE_T - 1);
+        const uint32_t g0 = fn_group[cm.grp_off + i], g1 = fn_group[cm.grp_off + i + 1];
+        ColView v;
+        v.m = &cm;
+        v.T = WIDE_T;
+        v.tb = WIDE_TB;
+        v.fn_c0 = fn_c0 + cm.fn_off + g0;
+        v.fn_delta = fn_delta + (size_t)(cm.fn_off + g0) * FN_STRIDE;
+        v.nf = g1 - g0;
+        v.prev = prev;
+        v.tab = nullptr;
+        v.tab_fn0 = 0;
+        v.prevm = prevm;
+        v.prevarg16 = prevarg;
+        key = wide_entry_key(v, o, i, (uint32_t)(gid & ((1ull << L) - 1)), L);
+    }
+    const uint32_t span = L < 5 ? 1u << L : 32u;
+    for (uint32_t off = 1; off < span; off <<= 1) {
+        const unsigned long long other = __shfl_xor_sync(0xFFFFFFFFu, key, off);
+        key = other < key ? other : key;
+    }
+    if ((threadIdx.x & (span - 1)) == 0 && e < nent) {
+        if (L <= 5) keys[e] = key;
+        else atomicMin(&keys[e], key);
+    }
+}
+
 // Backtrace on the device: the packed back-pointers stay in HBM, only the path comes back.
 // T == 1: DP-independent chains are traced by independent threads.
 __global__ void backtrace_kernel(const ColMeta *__restrict__ cols, const uint32_t *__restrict__ arena,
@@ -1134,6 +1201,8 @@ struct whmec_plan {
     DevBuf<uint32_t> d_fn_c0, d_fn_group, d_val[2], d_arena, d_chain_begin, d_path_index, d_path_tv, d_result;
     DevBuf<int32_t> d_fn_delta;
     DevBuf<unsigned long long> d_keys;
+    DevBuf<uint32_t> d_wide_m;   // wide sweep: the transformed previous projection and its argmins (wide_xform_kernel)
+    DevBuf<uint16_t> d_wide_arg;
     uint32_t last_buf = 0;
     ColPlan col;  // which column-kernel sweep, its memory-bounded segments and batched step lists (col_plan.h)
     // batched pedigree sweep (see col_batched_kernel)
@@ -1164,7 +1233,7 @@ struct whmec_plan {
         const bool healthy = !stream || cudaStreamSynchronize(stream) == cudaSuccess;
         d_cols.release(); d_fn_c0.release(); d_fn_group.release(); d_val[0].release(); d_val[1].release();
         d_arena.release(); d_chain_begin.release(); d_path_index.release(); d_path_tv.release();
-        d_result.release(); d_fn_delta.release(); d_keys.release();
+        d_result.release(); d_fn_delta.release(); d_keys.release(); d_wide_m.release(); d_wide_arg.release();
         d_ped_steps.release(); d_ped_vals.release(); d_chain_len.release(); d_ped_args.release();
         d_in_vec.release(); d_matrix.release(); d_bt_exits.release(); d_bt_entries.release();
         d_chain_rows.release(); d_chain_in.release(); d_chain_out.release();
@@ -1236,7 +1305,11 @@ int col_create(whmec_plan *pl, bool bounded_t1, uint64_t &h2d, std::string &msg)
     CUDA_TRY(up(pl->d_fn_delta.p, pk.fn_delta.data(), pk.fn_delta.size() * 4));
     CUDA_TRY(up(pl->d_fn_group.p, pk.fn_group.data(), pk.fn_group.size() * 4));
     CUDA_TRY(up(pl->d_chain_begin.p, pk.chain_begin.data(), pk.chain_begin.size() * 4));
-    pl->stats.path_kind = cp.path == ColPath::column ? 2 : 3;
+    pl->stats.path_kind = cp.path == ColPath::column ? 2 : cp.path == ColPath::wide ? 5 : 3;
+    if (cp.path == ColPath::wide) {
+        CUDA_TRY(pl->d_wide_m.alloc(cp.max_ent, pl->stream));
+        CUDA_TRY(pl->d_wide_arg.alloc(cp.max_ent, pl->stream));
+    }
     if (cp.path == ColPath::fused) {
         CUDA_TRY(pl->d_chain_rows.alloc((size_t)C * PF_T, pl->stream));
         CUDA_TRY(pl->d_chain_in.alloc((size_t)C * PF_T, pl->stream));
@@ -1275,6 +1348,10 @@ int plan_create_impl(const whmec_problem *p, int device, whmec_plan *pl, std::st
     else cudaGetLastError();
     pl->device = device;
     pl->segment = segment;
+    if (segment && p->n_trios > 4 && p->n_trios < p->n_ind) {  // (checked before packing: five-trio tables are large to pack)
+        msg = "unsupported: table segments are for pedigrees of at most 4 trio relationships (T <= 256); solve a five-trio table whole";
+        return WHMEC_ERR_UNSUPPORTED;
+    }
     // single-individual problems normally run on the tile kernel, which needs no per-read cost deltas
     const char *force = std::getenv("WHMEC_FORCE_COLUMN_KERNEL");  // test hook: exercise the general path on T == 1
     const bool forced_column = force && force[0] == '1';
@@ -1500,6 +1577,35 @@ int column_launch(whmec_plan *pl, uint32_t k, const uint32_t *prev, uint32_t *ou
     const uint32_t T = pk.T, tb = pk.tb;
     const ColMeta &m = pk.cols[k];
     const uint64_t nent = ((uint64_t)1 << m.f) * T;
+    if (pl->col.path == ColPath::wide) {
+        // transform (exact unless a sum can wrap), column step into keys, keys -> values and back-pointers
+        const bool xform = pk.nowrap;
+        if (xform) {
+            const uint64_t rows = m.first ? 1 : (uint64_t)1 << m.bw;
+            wide_xform_kernel<<<(unsigned)rows, WIDE_T, 0, pl->stream>>>(m.first ? nullptr : prev, m.rc, pl->d_wide_m.p, pl->d_wide_arg.p);
+            launches += 1;
+        }
+        const uint32_t L = wide_chunk_bits(m.f, m.d);
+        const uint64_t blocks = ((nent << L) + 255) / 256;
+        if (blocks > 0x7FFFFFFFull) {
+            if (capture) end_capture(pl);
+            msg = "unsupported: a column of this five-trio table has more candidates than one launch covers";
+            return WHMEC_ERR_UNSUPPORTED;
+        }
+        if (L > 5)
+            if (cudaError_t e = cudaMemsetAsync(pl->d_keys.p, 0xFF, nent * 8, pl->stream); e != cudaSuccess) {
+                if (capture) end_capture(pl);
+                msg = std::string("cudaMemsetAsync (wide column sweep): ") + cudaGetErrorString(e);
+                return WHMEC_ERR_CUDA;
+            }
+        ColMeta mk = m;
+        if (xform) mk.first = 0;  // (the first column's transform ran on zeros)
+        wide_step_kernel<<<(unsigned)blocks, 256, 0, pl->stream>>>(mk, pl->d_fn_c0.p, pl->d_fn_delta.p, pl->d_fn_group.p, prev,
+                                                                   xform ? pl->d_wide_m.p : nullptr, pl->d_wide_arg.p, L, pl->d_keys.p);
+        col_finalize_kernel<<<(unsigned)((nent + 255) / 256), 256, 0, pl->stream>>>(pl->d_cols.p, k, T, tb, pl->d_keys.p, out, pl->d_arena.p);
+        launches += 2;
+        return WHMEC_OK;
+    }
     if (m.d <= 6) {
         const uint32_t lc = col_lane_bits(m.f + tb, m.d);
         const uint64_t ent_per_block = 256u >> lc;

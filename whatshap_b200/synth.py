@@ -260,7 +260,7 @@ PEDIGREES = {
     "quartet": (4, [0, 1, 2, 0, 1, 3]),
     "three_generations": (5, [0, 1, 2, 2, 3, 4]),
     "three_children": (5, [0, 1, 2, 0, 1, 3, 0, 1, 4]),             # T = 64
-    "four_children": (6, [0, 1, 2, 0, 1, 3, 0, 1, 4, 0, 1, 5]),     # T = 256, the largest the path supports
+    "four_children": (6, [0, 1, 2, 0, 1, 3, 0, 1, 4, 0, 1, 5]),     # T = 256, the largest of the two-pass and genotyping paths (five trios: DESIGN §4.7)
 }
 
 
