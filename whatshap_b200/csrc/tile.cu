@@ -62,6 +62,9 @@ struct TileSmem {
     uint32_t cg[2];
     uint32_t a_col[TC_CHUNK];
     uint32_t panel_index;
+#ifdef WHMEC_TILE_PHASE_CLOCKS
+    unsigned long long phase_wait;  // thread 0's cycles in the column barrier's wait during the current work item
+#endif
 };
 static_assert(sizeof(TileSmem) <= 227 * 1024, "TileSmem exceeds the shared memory of one CTA on sm_90");
 
@@ -219,8 +222,13 @@ __device__ __forceinline__ void cp_async4(uint32_t *smem_dst, const uint32_t *gs
     const uint32_t d = (uint32_t)__cvta_generic_to_shared(smem_dst);
     asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(d), "l"(gsrc) : "memory");
 }
+__device__ __forceinline__ void cp_async16(void *smem_dst, const void *gsrc) {
+    const uint32_t d = (uint32_t)__cvta_generic_to_shared(smem_dst);
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d), "l"(gsrc) : "memory");
+}
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_group 0;" ::: "memory"); }
+__device__ __forceinline__ void cp_async_wait_1() { asm volatile("cp.async.wait_group 1;" ::: "memory"); }
 
 // ---- bulk asynchronous copies (TMA engine, cp.async.bulk) completing on an mbarrier
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -284,7 +292,13 @@ __device__ __forceinline__ void steady_columns(TileSmem &S, uint32_t ncol, uint3
             steady_prep<LG>(pr, S.scs[j + 1], S.TWs[j + 1][warp], S.T5s[j + 1][lane], S.buf[cur], S.buf[cur ^ 1], obase, pair_off, half, pop);
             bpw = arena + S.bp_at[j + 1];
         }
+#ifdef WHMEC_TILE_PHASE_CLOCKS
+        const long long w0 = clock64();
         mbar_wait(&S.col_bar, col_phase);
+        if (tid == 0) S.phase_wait += clock64() - w0;
+#else
+        mbar_wait(&S.col_bar, col_phase);
+#endif
         col_phase ^= 1u;
     }
 }
@@ -334,6 +348,23 @@ __device__ __forceinline__ void stage_tile_async(uint32_t *stage, const Panel *p
     cp_async_commit();
 }
 
+#ifdef WHMEC_TILE_PHASE_CLOCKS
+// Phase build (scripts/tile_phases.py only): thread 0 of every CTA records clock64() at the phase boundaries of each work
+// item -- start, input in place, tables built, columns done, end -- plus its cycles in the column barrier's wait.
+constexpr uint32_t PHASE_CAP = 1u << 20;  // records kept per collection; later work items are counted but not stored
+struct PhaseRec {
+    unsigned long long t[5];
+    unsigned long long wait;
+    uint32_t smid, block, steady, pad;
+};
+__device__ PhaseRec g_phase_rec[PHASE_CAP];
+__device__ unsigned int g_phase_n;
+#define WHMEC_PHASE(i) \
+    if (tid == 0) ph[i] = clock64()
+#else
+#define WHMEC_PHASE(i)
+#endif
+
 __global__ void __launch_bounds__(NT, 1)
 tile_panel_kernel(const Panel *__restrict__ panels, uint32_t n_panels, uint32_t total_tiles, int32_t tile_log, const TileCol *__restrict__ tcols,
                   const ColMeta *__restrict__ cols, uint32_t *__restrict__ state, uint32_t *__restrict__ arena,
@@ -354,6 +385,11 @@ tile_panel_kernel(const Panel *__restrict__ panels, uint32_t n_panels, uint32_t 
     }
     __syncthreads();
     for (uint32_t work = blockIdx.x; work < total_tiles; work += gridDim.x) {
+#ifdef WHMEC_TILE_PHASE_CLOCKS
+    unsigned long long ph[5];
+    WHMEC_PHASE(0);
+    if (tid == 0) S.phase_wait = 0;
+#endif
     if (tile_log >= 0) pi = work >> tile_log;  // every panel of this launch has 2^tile_log tiles
     else while (pi + 1 < n_panels && __ldg(&panels[pi + 1].tile_begin) <= work) ++pi;
     __syncthreads();  // previous work item completely done (its stores read the buffers, S.P is reused)
@@ -362,6 +398,28 @@ tile_panel_kernel(const Panel *__restrict__ panels, uint32_t n_panels, uint32_t 
     const Panel &P = S.P;
     const uint32_t tile = work - P.tile_begin;
     uint32_t cur = 0;
+    // Steady-state panels: their column descriptors start streaming into shared memory now, under the wait for the input.
+    if (P.steady) {
+        static_assert(sizeof(TileCol) % 16 == 0, "TileCol records are copied in 16-byte pieces");
+        constexpr uint32_t CHUNKS = sizeof(TileCol) / 16;
+        if (tid < (P.col_end - P.col_begin) * CHUNKS)
+            cp_async16(reinterpret_cast<uint4 *>(S.tcs) + tid, reinterpret_cast<const uint4 *>(tcols + P.col_begin) + tid);
+        cp_async_commit();
+    }
+    // Where the input of this CTA's next tile comes from (prefetched below, once the staging buffer is free): looked up now,
+    // so that these loads are in flight under the input wait.  next = (panel << 2) | mode, mode 0 = nothing to prefetch,
+    // 1 = cp.async gather, 2 = bulk copies.
+    uint32_t next = 0;
+    {
+        const uint32_t nwork = work + gridDim.x;
+        if (nwork < total_tiles) {
+            uint32_t pn = pi;
+            if (tile_log >= 0) pn = nwork >> tile_log;
+            else while (pn + 1 < n_panels && __ldg(&panels[pn + 1].tile_begin) <= nwork) ++pn;
+            if (__ldg(&panels[pn].in_layout) == 1 && !__ldg(&panels[pn].fresh))
+                next = (pn << 2) | (bulk_handoff(__ldg(&panels[pn].in_gA), __ldg(&panels[pn].in_j)) ? 2u : 1u);
+        }
+    }
 
     // ---- the tile's slice of the incoming projection column
     if (P.fresh) {
@@ -421,38 +479,29 @@ tile_panel_kernel(const Panel *__restrict__ panels, uint32_t n_panels, uint32_t 
         }
     }
     __syncthreads();  // staging buffer free again
+    WHMEC_PHASE(1);
     // ---- prefetch the input of this CTA's next tile
-    staged = 0;
-    {
-        const uint32_t nwork = work + gridDim.x;
-        if (nwork < total_tiles) {
-            uint32_t pn = pi;
-            if (tile_log >= 0) pn = nwork >> tile_log;
-            else while (pn + 1 < n_panels && __ldg(&panels[pn + 1].tile_begin) <= nwork) ++pn;
-            if (__ldg(&panels[pn].in_layout) == 1 && !__ldg(&panels[pn].fresh)) {
-                const uint32_t ntile = nwork - __ldg(&panels[pn].tile_begin);
-                if (bulk_handoff(__ldg(&panels[pn].in_gA), __ldg(&panels[pn].in_j))) {
-                    if (tid < 32) {
-                        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic reads of the buffer above -> async writes
-                        stage_tile_bulk(S.buf[2], &S.stage_bar, &panels[pn], ntile, state);
-                    }
-                    staged = 2;
-                } else {
-                    stage_tile_async(S.buf[2], &panels[pn], ntile, state);
-                    staged = 1;
-                }
+    staged = next & 3u;
+    if (staged) {
+        const Panel *pn = &panels[next >> 2];
+        const uint32_t ntile = work + gridDim.x - __ldg(&pn->tile_begin);
+        if (staged == 2) {
+            if (tid < 32) {
+                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic reads of the buffer above -> async writes
+                stage_tile_bulk(S.buf[2], &S.stage_bar, pn, ntile, state);
             }
+        } else {
+            stage_tile_async(S.buf[2], pn, ntile, state);
         }
     }
 
     if (P.steady) {
         // ---- steady-state panel: every column is the twin fast column of one tile size.  Descriptors and ALL tables of
-        // the panel are built once, in parallel (thread (column, entry)); then one barrier and one call per column.
-        const uint32_t kb = P.col_begin, ncol = P.col_end - kb;
-        {
-            constexpr uint32_t WORDS = sizeof(TileCol) / 4;
-            for (uint32_t w = tid; w < ncol * WORDS; w += NT) ((uint32_t *)S.tcs)[w] = ((const uint32_t *)(tcols + kb))[w];
-        }
+        // the panel are built once, in parallel (thread (column, entry)); then one barrier and one call per column.  The
+        // descriptors were requested when the work item started (cp.async above).
+        const uint32_t ncol = P.col_end - P.col_begin;
+        if (staged == 1) cp_async_wait_1();  // the descriptors' group; the next tile's gather (the newest group) stays in flight
+        else cp_async_wait_all();
         __syncthreads();
         {
             const uint32_t j = tid >> 6, idx = tid & 63u;
@@ -470,6 +519,7 @@ tile_panel_kernel(const Panel *__restrict__ panels, uint32_t n_panels, uint32_t 
         const bool mirror = S.tcs[0].half && S.tcs[0].km != 0;
         const uint32_t lg = P.steady - 1u;
         __syncthreads();  // tables ready; the tile's input is in place
+        WHMEC_PHASE(2);
         if (lg == 3) {
             if (mirror) steady_columns<3, true>(S, ncol, arena, cur, col_phase, tid);
             else steady_columns<3, false>(S, ncol, arena, cur, col_phase, tid);
@@ -477,7 +527,8 @@ tile_panel_kernel(const Panel *__restrict__ panels, uint32_t n_panels, uint32_t 
             if (mirror) steady_columns<2, true>(S, ncol, arena, cur, col_phase, tid);
             else steady_columns<2, false>(S, ncol, arena, cur, col_phase, tid);
         }
-    } else
+    } else {
+    WHMEC_PHASE(2);  // other panels build their tables column by column inside the loop
     for (uint32_t k = P.col_begin; k < P.col_end; ++k) {
         const uint32_t j = (k - P.col_begin) % TC_CHUNK;
         if (j == 0) {
@@ -613,6 +664,8 @@ tile_panel_kernel(const Panel *__restrict__ panels, uint32_t n_panels, uint32_t 
             cur ^= 1;
         }
     }
+    }
+    WHMEC_PHASE(3);
 
     // ---- write the tile back in canonical layout for the next panel
     if (!P.ends_chain && P.out_layout == 1) {
@@ -635,6 +688,23 @@ tile_panel_kernel(const Panel *__restrict__ panels, uint32_t n_panels, uint32_t 
         uint32_t *dst = state + P.out_off;
         for (uint32_t l = tid, it = 0; l < nout; l += NT, ++it) dst[lo | pdep32(it, himask) | gpart] = S.buf[cur][l];
     }
+#ifdef WHMEC_TILE_PHASE_CLOCKS
+    WHMEC_PHASE(4);
+    if (tid == 0) {
+        const uint32_t slot = atomicAdd(&g_phase_n, 1u);
+        if (slot < PHASE_CAP) {
+            PhaseRec &r = g_phase_rec[slot];
+            for (int i = 0; i < 5; ++i) r.t[i] = ph[i];
+            r.wait = S.phase_wait;
+            uint32_t smid;
+            asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
+            r.smid = smid;
+            r.block = blockIdx.x;
+            r.steady = P.steady;
+            r.pad = 0;
+        }
+    }
+#endif
     }  // work loop
 }
 
@@ -978,3 +1048,19 @@ void TilePlan::release(cudaStream_t stream) {
 }
 
 }  // namespace whmec
+
+#ifdef WHMEC_TILE_PHASE_CLOCKS
+// Phase build only: start a new collection / copy the records collected since (8 x u64 each).  Returns the number of work
+// items seen, which exceeds `cap` (and PHASE_CAP) when records were dropped.
+extern "C" int whmec_tile_phase_reset(void) {
+    const unsigned int zero = 0;
+    return cudaMemcpyToSymbol(whmec::g_phase_n, &zero, sizeof zero) == cudaSuccess ? 0 : -1;
+}
+extern "C" long long whmec_tile_phase_read(void *out, unsigned long long cap) {
+    unsigned int n = 0;
+    if (cudaDeviceSynchronize() != cudaSuccess || cudaMemcpyFromSymbol(&n, whmec::g_phase_n, sizeof n) != cudaSuccess) return -1;
+    const unsigned long long keep = std::min<unsigned long long>({n, cap, whmec::PHASE_CAP});
+    if (keep && cudaMemcpyFromSymbol(out, whmec::g_phase_rec, keep * sizeof(whmec::PhaseRec)) != cudaSuccess) return -1;
+    return n;
+}
+#endif
