@@ -23,7 +23,7 @@ from typing import List, Optional, Sequence, Tuple
 
 import numpy as np
 
-from . import _lib
+from . import _lib, multigpu
 from ._abi import GT_OTHER, FlatProblem
 
 
@@ -207,14 +207,15 @@ def flatten_objects(readset, recombcost, pedigree, distrust_genotypes: bool = Fa
 def make_dp_table_class(core_module, solver=None):
     """A `PedigreeDPTable` look-alike (same constructor, same three methods, `whatshap/types.py:7-15`)
     that solves on the GPU and answers with `core_module`'s own Read / ReadSet objects.
-    `solver(problem) -> FlatSolution` defaults to the CUDA path; tests may inject a CPU checker."""
+    `solver(problem) -> FlatSolution` defaults to the CUDA path: device 0, or every GPU listed in WHMEC_DEVICES
+    (`multigpu.solve_table`); tests may inject a CPU checker."""
     Read, ReadSet = core_module.Read, core_module.ReadSet
 
     class PedigreeDPTable:
         def __init__(self, readset, recombcost, pedigree, distrust_genotypes=False, positions=None):
             self.pedigree = pedigree
             self._problem, self._ids = flatten_objects(readset, recombcost, pedigree, distrust_genotypes, positions)
-            solve = solver or (lambda p: _lib.solve(p)[0])
+            solve = solver or (lambda p: multigpu.solve_table(p)[0])
             self._solution = solve(self._problem)
 
         def get_super_reads(self):
@@ -294,7 +295,8 @@ def make_genotype_table_class(core_module, solver=None):
     """A `GenotypeDPTable` look-alike (constructor and `get_genotype_likelihoods` of whatshap/core.pyx:581-600) that
     runs the forward-backward DP on the GPU from `core_module`'s own objects and answers with its
     `PhredGenotypeLikelihoods`.  The pedigree should be a `recording_pedigree` (exact genotype priors; the `str()`
-    fallback keeps 6 significant digits).  `solver(problem) -> ndarray [n_ind, n_cols, 3]` defaults to the CUDA path."""
+    fallback keeps 6 significant digits).  `solver(problem) -> ndarray [n_ind, n_cols, 3]` defaults to the CUDA path: device
+    0, or every GPU listed in WHMEC_DEVICES (`multigpu.genotype_table`)."""
     Likelihoods = core_module.PhredGenotypeLikelihoods
 
     class GenotypeDPTable:
@@ -303,7 +305,7 @@ def make_genotype_table_class(core_module, solver=None):
             self.numeric_sample_ids = numeric_sample_ids
             # the priors travel where distrusted genotypes carry their likelihoods
             self._problem, self._ids = flatten_objects(readset, recombcost, pedigree, True, positions)
-            run = solver or (lambda p: _lib.genotype(p)[0])
+            run = solver or (lambda p: multigpu.genotype_table(p)[0])
             self._likelihoods = run(self._problem)
 
         def get_genotype_likelihoods(self, sample_id, pos):

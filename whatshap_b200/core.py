@@ -18,7 +18,7 @@ from typing import Dict, Iterable, Iterator, List, Optional, Sequence, Tuple
 
 import numpy as np
 
-from . import _lib
+from . import _lib, multigpu
 from ._abi import GT_OTHER, FlatProblem, FlatSolution
 from .variant import Variant
 
@@ -741,17 +741,19 @@ def _flatten(readset: ReadSet, recombcost: Sequence[int], pedigree: Pedigree, di
 
 class PedigreeDPTable:
     """Exact weighted-MEC / PedMEC solver; the constructor does all the work
-    (core.pyx:364-416; abstract contract whatshap/types.py:7-15)."""
+    (core.pyx:364-416; abstract contract whatshap/types.py:7-15).  `devices` (CUDA ordinals; default: those of
+    WHMEC_DEVICES if it is set) spreads the table over several GPUs from this process (`multigpu.solve_on_devices`) with
+    the same result; otherwise it runs on `device`."""
 
     def __init__(self, readset: ReadSet, recombcost, pedigree: Pedigree, distrust_genotypes: bool = False,
-                 positions=None, device: int = 0):
+                 positions=None, device: int = 0, devices=None):
         if not isinstance(readset, ReadSet):
             raise TypeError("Argument 'readset' has incorrect type")
         if not isinstance(pedigree, Pedigree):
             raise TypeError("Argument 'pedigree' has incorrect type")
         self.pedigree = pedigree
         self._problem = _flatten(readset, recombcost, pedigree, bool(distrust_genotypes), positions)
-        self._solution, self.stats = _lib.solve(self._problem, device=device)
+        self._solution, self.stats = multigpu.solve_table(self._problem, device, devices)
 
     def get_super_reads(self) -> Tuple[List[ReadSet], List[int]]:
         """One ReadSet per individual (pedigree order) holding `superread_0_<k>` and
@@ -859,10 +861,11 @@ class PedMecHeuristic:
 class GenotypeDPTable:
     """Genotype likelihoods by the forward-backward algorithm over the same bipartition DP; the constructor
     does all the work (core.pyx:581-600, src/genotypedptable.cpp:17-48).  `pedigree` must carry genotype
-    likelihoods (priors) for every variant; `recombcost` are phred-scaled recombination probabilities."""
+    likelihoods (priors) for every variant; `recombcost` are phred-scaled recombination probabilities.  `device` /
+    `devices` as for `PedigreeDPTable` (`multigpu.genotype_on_devices`)."""
 
     def __init__(self, numeric_sample_ids: NumericSampleIds, readset: ReadSet, recombcost, pedigree: Pedigree,
-                 positions=None, device: int = 0):
+                 positions=None, device: int = 0, devices=None):
         if not isinstance(readset, ReadSet):
             raise TypeError("Argument 'readset' has incorrect type")
         if not isinstance(pedigree, Pedigree):
@@ -871,7 +874,7 @@ class GenotypeDPTable:
         self.numeric_sample_ids = numeric_sample_ids
         # the priors travel in the `gl` array of the flat problem (as they do for distrusted genotypes)
         self._problem = _flatten(readset, recombcost, pedigree, True, positions)
-        self._likelihoods, self.stats = _lib.genotype(self._problem, device=device)
+        self._likelihoods, self.stats = multigpu.genotype_table(self._problem, device, devices)
 
     def get_genotype_likelihoods(self, sample_id, pos: int) -> PhredGenotypeLikelihoods:
         """Likelihoods of 0/0, 0/1, 1/1 of `sample_id` at column `pos` (src/genotypedptable.cpp:445-451)."""

@@ -12,6 +12,10 @@ forward-backward genotyping DP of a single individual, and by segments of the ta
 segment (`whmec_genotype_segment_*`), the ranks all-gather T x T transfer matrices of doubles, fold them into every
 segment's true forward and backward inputs, and each runs its segment (DESIGN §4.5).
 
+`solve_on_devices` / `genotype_on_devices` make the same cuts in ONE process (no process group): one host thread per
+device, the folds on the calling thread.  `core`'s tables and the swap-in classes of `adapters` reach them through
+`solve_table` / `genotype_table` when given `devices` or when WHMEC_DEVICES is set (DESIGN §6).
+
 The reference has no counterpart (single process, `whatshap/cli/phase.py:604-610` runs one
 PedigreeDPTable per chromosome x family).
 """
@@ -194,6 +198,24 @@ def segment_ranges(prob: FlatProblem, world: int) -> List[Optional[Tuple[int, in
     return [(blocks[b0][0], blocks[b1 - 1][1]) if b1 > b0 else None for b0, b1 in shares]
 
 
+def plan_parts(prob: FlatProblem, world: int, genotype: bool = False, spans=None
+               ) -> Tuple[str, List[Optional[Tuple[int, int]]]]:
+    """How a table is cut over `world` devices, for every driver (`solve_sharded`, `genotype_sharded`, `solve_on_devices`,
+    `genotype_on_devices`).  Returns (mode, ranges):
+      "whole"    -- the table on one device (ranges empty): no columns, or a pedigree of one chain, or one device for a pedigree;
+      "blocks"   -- a single individual (T = 1): device i takes a contiguous run of whole chains with about 1 / world of the DP cells;
+      "segments" -- a pedigree of two chains or more: device i holds a segment of the table (`segment_ranges`).
+    `ranges[i]` is device i's column range [lo, hi), None when it holds no columns.  Genotyping also runs a single individual
+    whole on one device instead of as one run of blocks.  `spans`: the reads' column spans (`_read_spans`) if known."""
+    if prob.n_cols == 0 or (genotype and world == 1):
+        return "whole", []
+    blocks = independent_blocks(prob, spans)
+    if prob.n_trios > 0:  # transmission vectors couple the chains: segments of the table, or the whole table on one device
+        return ("segments", segment_ranges(prob, world)) if world > 1 and len(blocks) > 1 else ("whole", [])
+    runs = contiguous_shares(block_work(prob, blocks, spans), world)
+    return "blocks", [(blocks[b0][0], blocks[b1 - 1][1]) if b1 > b0 else None for b0, b1 in runs]
+
+
 def solve_pedigree_segments(prob: FlatProblem, n_segments: int, segment_factory=None) -> FlatSolution:
     """The multi-GPU pedigree scheme with all `n_segments` segments driven by ONE process on one
     device, in the order the ranks would run them -- the single-GPU check of `whmec_segment_*`
@@ -318,24 +340,20 @@ def solve_sharded(prob: Optional[FlatProblem], solver: Optional[Callable[[FlatPr
     rank, world = comm.rank, comm.world
     t0 = time.perf_counter()
     rows = None
-    blocks = None
-    MODE = {"single": 0, "blocks": 1, "segments": 2}
+    MODE = {"whole": 0, "blocks": 1, "segments": 2}
     if rank == 0:
         spans = _read_spans(prob) if prob.n_reads else None
-        blocks = independent_blocks(prob, spans)
-        if prob.n_trios > 0 and world > 1 and len(blocks) > 1:  # transmission vectors couple the blocks: segments of the table
-            ranges = segment_ranges(prob, world)
+        mode, ranges = plan_parts(prob, world, spans=spans)
+        if mode == "segments":
             flat = np.array([MODE["segments"]] + [x for r in ranges for x in (r if r is not None else (0, 0))], np.int64)
             rows = [[flat.view(np.uint8)] + ([enc] if enc is not None else []) for enc in _wire.encode_problem_slices(prob, ranges)]
-        elif prob.n_trios > 0 or prob.n_cols == 0:  # one chain, one rank, or no columns: one GPU
-            rows = [[np.array([MODE["single"]], np.int64).view(np.uint8)]] * world
+        elif mode == "whole":
+            rows = [[np.array([MODE["whole"]], np.int64).view(np.uint8)]] * world
         else:
             # every rank gets ONE sub-problem: a contiguous run of whole blocks with about 1 / world of the DP cells (one
             # whmec_solve per rank sweeps all its chains together; block-by-block calls would be launch-latency bound)
-            runs = contiguous_shares(block_work(prob, blocks, spans), world)
-            cuts = [(blocks[b0][0], blocks[b1 - 1][1]) if b1 > b0 else None for b0, b1 in runs]
             rows = [[np.array([MODE["blocks"]], np.int64).view(np.uint8)] + ([enc] if enc is not None else [])
-                    for enc in _wire.encode_problem_slices(prob, cuts)]
+                    for enc in _wire.encode_problem_slices(prob, ranges)]
     t1 = time.perf_counter()
     pieces = _wire.separate(comm.scatter_rows(rows))
     head = pieces[0].view(np.int64)
@@ -349,8 +367,8 @@ def solve_sharded(prob: Optional[FlatProblem], solver: Optional[Callable[[FlatPr
         handled, sol = solve_pedigree_sharded(prob, segment_factory, group, ranges=ranges, my_slice=piece, comm=comm, timings=timings)
         if handled:
             return sol
-        mode = MODE["single"]  # some segment is outside the two-pass scheme: the whole table on rank 0's GPU
-    if mode == MODE["single"]:
+        mode = MODE["whole"]  # some segment is outside the two-pass scheme: the whole table on rank 0's GPU
+    if mode == MODE["whole"]:
         sol, err = None, None
         if rank == 0:
             try:
@@ -473,20 +491,14 @@ def genotype_sharded(prob: Optional[FlatProblem], solver: Optional[Callable[[Fla
     rank, world = comm.rank, comm.world
     rows = None
     if rank == 0:
-        blocks = independent_blocks(prob) if prob.n_cols and world > 1 else []
-        if prob.n_trios > 0 and len(blocks) > 1:  # transmission vectors couple the chains: segments of the table
-            rows = []
-            for r in segment_ranges(prob, world):
-                lo, hi = r if r is not None else (0, 0)
-                rows.append(_wire.join([np.array([2, lo, hi, prob.n_cols], np.int64).view(np.uint8)] +
-                                       ([_wire.encode_problem(prob.slice_columns(lo, hi), lo=lo)] if hi > lo else [])))
-        elif prob.n_trios > 0 or prob.n_cols == 0 or world == 1:
+        plan, ranges = plan_parts(prob, world, genotype=True)
+        if plan == "whole":
             rows = [_wire.join([np.array([0, 0, 0, 0], np.int64).view(np.uint8)])] * world
-        else:  # every rank receives only its run of chains
+        else:  # every rank receives only its run of chains or its segment of the table
             rows = []
-            for b0, b1 in contiguous_shares(block_work(prob, blocks), world):
-                lo, hi = (blocks[b0][0], blocks[b1 - 1][1]) if b1 > b0 else (0, 0)
-                rows.append(_wire.join([np.array([1, lo, hi, prob.n_cols], np.int64).view(np.uint8)] +
+            for r in ranges:
+                lo, hi = r if r is not None else (0, 0)
+                rows.append(_wire.join([np.array([2 if plan == "segments" else 1, lo, hi, prob.n_cols], np.int64).view(np.uint8)] +
                                        ([_wire.encode_problem(prob.slice_columns(lo, hi), lo=lo)] if hi > lo else [])))
     pieces = _wire.separate(comm.scatter_rows(rows))
     mode, lo, hi, n_cols = (int(x) for x in pieces[0].view(np.int64))
@@ -564,3 +576,252 @@ def _genotype_segment_rank(row: Optional[np.ndarray], lo: int, hi: int, n_cols: 
         if seg is not None:
             seg.close()
     return True, out
+
+
+# ---- one process, several devices ---------------------------------------------------------------------------------
+#
+# The same cuts and folds as the distributed drivers above, for a caller that is a single process (`whatshap phase` and
+# `whatshap genotype` build one table at a time): one host thread per distinct device runs that device's parts through the
+# C ABI, which is re-entrant, sets the device on the calling thread and releases the GIL (ctypes); the folds between
+# phases run on the calling thread.
+
+ENV_DEVICES = "WHMEC_DEVICES"
+
+
+def _run_on_devices(devices: Sequence[int], jobs: Sequence[Optional[Callable[[], object]]]) -> Tuple[list, list]:
+    """Runs `jobs[i]()` (None: nothing to do) on the host thread of `devices[i]`, one thread per distinct device, so that
+    all devices work at once; the jobs of one device run one after another in list order (two plans created at once on one
+    device would each size their arena from the same free HBM).  Returns (results, errors), one entry per job, after every
+    thread has been joined."""
+    import threading
+
+    results: list = [None] * len(jobs)
+    errors: list = [None] * len(jobs)
+    lanes: dict = {}
+    for i, d in enumerate(devices):
+        lanes.setdefault(d, []).append(i)
+
+    def lane(indices):
+        for i in indices:
+            if jobs[i] is not None:
+                try:
+                    results[i] = jobs[i]()
+                except Exception as e:  # noqa: BLE001 - raised on the calling thread, lowest column first
+                    errors[i] = e
+
+    threads = [threading.Thread(target=lane, args=(indices,), name="whmec-device-%d" % d) for d, indices in lanes.items()]
+    for t in threads:
+        t.start()
+    for t in threads:
+        t.join()
+    return results, errors
+
+
+def _raise_first(errors: Sequence[Optional[BaseException]], refusals_fall_back: bool) -> bool:
+    """Raises the error of the part with the lowest column (the parts are in column order).  With `refusals_fall_back` a
+    refusal (Unsupported) is not raised but reported: returns True if some part was refused, as `_wire.raise_first_error`
+    does for the ranks of the distributed drivers."""
+    from ._abi import Unsupported
+
+    for e in errors:
+        if e is not None and not (refusals_fall_back and isinstance(e, Unsupported)):
+            raise e
+    return any(isinstance(e, Unsupported) for e in errors)
+
+
+def _segment_stats(seg) -> dict:
+    st = getattr(seg, "stats", None)  # `_lib.Segment.stats()`, `_lib.GenotypeSegment.stats` (its last call)
+    return dict(st() if callable(st) else st or {})
+
+
+def _whole_stats(n_cols: int, devices: Sequence[int], st) -> dict:
+    return {"mode": "whole", "devices": list(devices), "parts": [{"device": devices[0], "columns": (0, n_cols), "stats": dict(st or {})}]}
+
+
+def _part_stats(mode: str, devices: Sequence[int], ranges, stats) -> dict:
+    return {"mode": mode, "devices": list(devices),
+            "parts": [{"device": d, "columns": r, "stats": st} for d, r, st in zip(devices, ranges, stats) if r is not None]}
+
+
+def solve_on_devices(prob: FlatProblem, devices: Sequence[int], solver=None, segment_factory=None) -> Tuple[FlatSolution, dict]:
+    """`solve_sharded` in one process: one part of `prob` per entry of `devices`, in column order (`plan_parts`); the
+    same solution as `whmec_solve` on one device.  A single individual is cut into runs of whole chains, each solved by
+    `solver(part, device)`; a pedigree of two chains or more into segments of the table, driven phase by phase (create,
+    transfer, `segment_inputs`, sweep, exits, `segment_entries`, finish, `merge_block_solutions`).  Runs whole on
+    `devices[0]`: a pedigree of one chain, a problem without columns, and a table some segment of which is refused as
+    unsupported while it is created or run.  An error is raised after every part has stopped and every segment is closed:
+    that of the part with the lowest column (a refusal only when the whole table is refused too).  A device may repeat:
+    its parts run one after another.  `solver(prob, device) -> (FlatSolution, stats)` defaults to `_lib.solve`,
+    `segment_factory(prob, continues, device)` to `_lib.Segment`.  Returns (solution, stats): the mode, the devices and
+    every part's device, column range and statistics."""
+    from . import _lib
+
+    devices = [int(d) for d in devices]
+    solver = solver or _lib.solve
+    factory = segment_factory or _lib.Segment
+    mode, ranges = plan_parts(prob, len(devices))
+    if mode == "blocks":
+        jobs = [None if r is None else (lambda r=r, d=d: solver(prob.slice_columns(*r), d)) for r, d in zip(ranges, devices)]
+        done, errors = _run_on_devices(devices, jobs)
+        _raise_first(errors, False)
+        parts = [(r, out) for r, out in zip(ranges, done) if r is not None]
+        return (merge_block_solutions(prob, [r for r, _ in parts], [out[0] for _, out in parts]),
+                _part_stats(mode, devices, ranges, [None if out is None else dict(out[1] or {}) for out in done]))
+    if mode == "segments":
+        done = _solve_segments(prob, devices, ranges, factory)
+        if done is not None:
+            return done
+    sol, st = solver(prob, devices[0])
+    return sol, _whole_stats(prob.n_cols, devices, st)
+
+
+def _solve_segments(prob: FlatProblem, devices: List[int], ranges, factory) -> Optional[Tuple[FlatSolution, dict]]:
+    """The segment mode of `solve_on_devices`; None when some segment is refused as unsupported."""
+    segs: list = [None] * len(ranges)
+    last_active = max(i for i, r in enumerate(ranges) if r is not None)
+
+    def phase(step):
+        """step(i, segment) on the thread of every part that holds a segment; True if one was refused."""
+        out, errors = _run_on_devices(devices, [None if sg is None else (lambda i=i, sg=sg: step(i, sg)) for i, sg in enumerate(segs)])
+        return out, _raise_first(errors, True)
+
+    try:
+        segs, errors = _run_on_devices(devices, [None if r is None else (lambda r=r, d=d: factory(prob.slice_columns(*r), r[0] > 0, d))
+                                                 for r, d in zip(ranges, devices)])
+        if _raise_first(errors, True):
+            return None
+        matrices, refused = phase(lambda i, sg: sg.transfer())
+        if refused:
+            return None
+        inputs = segment_inputs(matrices)
+        if phase(lambda i, sg: sg.sweep(inputs[i]))[1]:
+            return None
+        exits, refused = phase(lambda i, sg: sg.exits(i == last_active))
+        if refused:
+            return None
+        entries = segment_entries(exits)
+        done, refused = phase(lambda i, sg: (sg.finish(entries[i]), _segment_stats(sg)))
+        if refused:
+            return None
+    finally:
+        _run_on_devices(devices, [None if sg is None else sg.close for sg in segs])
+    parts = [(r, out[0]) for r, out in zip(ranges, done) if out is not None]
+    sol = merge_block_solutions(prob, [r for r, _ in parts], [s for _, s in parts], cost=int(parts[-1][1].cost))
+    return sol, _part_stats("segments", devices, ranges, [None if out is None else out[1] for out in done])
+
+
+def genotype_on_devices(prob: FlatProblem, devices: Sequence[int], solver=None, segment_factory=None) -> Tuple[np.ndarray, dict]:
+    """`genotype_sharded` in one process: likelihoods [n_ind, n_cols, 3] with one part of `prob` per entry of `devices`, in
+    column order (`plan_parts`).  A single individual is cut into runs of whole chains, each genotyped by
+    `solver(part, device)`; a pedigree of two chains or more into segments of the table (create, transfer,
+    `genotype_segment_inputs`, run).  Runs whole on `devices[0]`: one device, a pedigree of one chain, a problem without
+    columns, and a table some segment of which is refused as unsupported while it is created, transferred or run.  Errors,
+    repeated devices and the result's statistics as in `solve_on_devices`.  `solver(prob, device) -> (likelihoods, stats)`
+    defaults to `_lib.genotype`, `segment_factory(prob, continues, continued, device)` to `_lib.GenotypeSegment`."""
+    from . import _lib
+
+    devices = [int(d) for d in devices]
+    solver = solver or _lib.genotype
+    factory = segment_factory or _lib.GenotypeSegment
+    mode, ranges = plan_parts(prob, len(devices), genotype=True)
+    if mode == "blocks":
+        jobs = [None if r is None else (lambda r=r, d=d: solver(prob.slice_columns(*r), d)) for r, d in zip(ranges, devices)]
+        done, errors = _run_on_devices(devices, jobs)
+        _raise_first(errors, False)
+        out = np.zeros((prob.n_ind, prob.n_cols, 3), np.float64)
+        for r, part in zip(ranges, done):
+            if r is not None:
+                out[:, r[0]:r[1], :] = part[0]
+        return out, _part_stats(mode, devices, ranges, [None if part is None else dict(part[1] or {}) for part in done])
+    if mode == "segments":
+        done = _genotype_segments(prob, devices, ranges, factory)
+        if done is not None:
+            return done
+    out, st = solver(prob, devices[0])
+    return out, _whole_stats(prob.n_cols, devices, st)
+
+
+def _genotype_segments(prob: FlatProblem, devices: List[int], ranges, factory) -> Optional[Tuple[np.ndarray, dict]]:
+    """The segment mode of `genotype_on_devices`; None when some segment is refused as unsupported."""
+    segs: list = [None] * len(ranges)
+    n = prob.n_cols
+
+    def phase(step):
+        out, errors = _run_on_devices(devices, [None if sg is None else (lambda i=i, sg=sg: step(i, sg)) for i, sg in enumerate(segs)])
+        return out, _raise_first(errors, True)
+
+    try:
+        segs, errors = _run_on_devices(devices, [None if r is None else (lambda r=r, d=d: factory(prob.slice_columns(*r), r[0] > 0, r[1] < n, d))
+                                                 for r, d in zip(ranges, devices)])
+        if _raise_first(errors, True):
+            return None
+        transfers, refused = phase(lambda i, sg: (sg.transfer(), _segment_stats(sg)))
+        if refused:
+            return None
+        alphas, betas = genotype_segment_inputs([None if t is None else t[0] for t in transfers])
+        runs, refused = phase(lambda i, sg: (sg.run(alphas[i], betas[i]), _segment_stats(sg)))
+        if refused:
+            return None
+    finally:
+        _run_on_devices(devices, [None if sg is None else sg.close for sg in segs])
+    out = np.zeros((prob.n_ind, n, 3), np.float64)
+    for r, run in zip(ranges, runs):
+        if run is not None:
+            out[:, r[0]:r[1], :] = run[0]
+    stats = [None if t is None else {"transfer": t[1], "run": run[1]} for t, run in zip(transfers, runs)]
+    return out, _part_stats("segments", devices, ranges, stats)
+
+
+def parse_devices(text: str) -> List[int]:
+    """The CUDA ordinals of a WHMEC_DEVICES value ("0,1,2,3"); ValueError naming the variable when it is malformed."""
+    items = [t.strip() for t in text.split(",")]
+    if not all(t.isascii() and t.isdigit() for t in items):
+        raise ValueError("%s=%r: expected comma-separated CUDA device ordinals, e.g. 0,1,2,3" % (ENV_DEVICES, text))
+    return [int(t) for t in items]
+
+
+def table_devices(device: int = 0, devices: Optional[Sequence[int]] = None) -> Optional[List[int]]:
+    """The devices one table runs on: `devices`, else the ordinals of WHMEC_DEVICES, else None (the table runs on `device`
+    alone, as before there was a choice).  A non-default `device` is kept over WHMEC_DEVICES: code that names a device
+    runs there.  ValueError for both a non-default `device` and `devices`, an empty list, a malformed WHMEC_DEVICES and an
+    ordinal that is not a visible CUDA device."""
+    import os
+
+    from . import _lib
+
+    if devices is not None and device != 0:
+        raise ValueError("give either device=%r or devices=%r, not both" % (device, devices))
+    if devices is None:
+        text = os.environ.get(ENV_DEVICES, "").strip()
+        if not text or device != 0:
+            return None
+        devices = parse_devices(text)
+    chosen = list(devices)
+    if not chosen:
+        raise ValueError("devices: expected at least one CUDA device ordinal")
+    count = None
+    for d in chosen:
+        if isinstance(d, bool) or not isinstance(d, (int, np.integer)) or d < 0:
+            raise ValueError("device ordinal %r is not a non-negative integer" % (d,))
+        count = _lib.device_count() if count is None else count
+        if d >= count:
+            raise ValueError("device ordinal %d is not a visible CUDA device (%d visible)" % (d, count))
+    return [int(d) for d in chosen]
+
+
+def solve_table(prob: FlatProblem, device: int = 0, devices: Optional[Sequence[int]] = None) -> Tuple[FlatSolution, dict]:
+    """What `core.PedigreeDPTable` and the swap-in class of `adapters` run: `_lib.solve` on `device`, or
+    `solve_on_devices` over `devices` / WHMEC_DEVICES (`table_devices`)."""
+    from . import _lib
+
+    chosen = table_devices(device, devices)
+    return _lib.solve(prob, device=device) if chosen is None else solve_on_devices(prob, chosen)
+
+
+def genotype_table(prob: FlatProblem, device: int = 0, devices: Optional[Sequence[int]] = None) -> Tuple[np.ndarray, dict]:
+    """What `core.GenotypeDPTable` and the swap-in class of `adapters` run: `_lib.genotype` on `device`, or
+    `genotype_on_devices` over `devices` / WHMEC_DEVICES (`table_devices`)."""
+    from . import _lib
+
+    chosen = table_devices(device, devices)
+    return _lib.genotype(prob, device=device) if chosen is None else genotype_on_devices(prob, chosen)
