@@ -8,11 +8,13 @@ every CTA of tile_panel_kernel records clock64() at five points of each work ite
 
     start -> input in place -> tables built -> columns done -> end of the item
 
-plus the cycles it spends waiting at the column barrier of steady-state panels.  The normal build's SASS does not change:
+plus the cycles it spends waiting at the column barrier of steady-state panels and waiting for the completion counter of
+the producer panel (an input that was not prefetched).  The normal build's SASS does not change:
 every line the macro adds is inside #ifdef.  For each workload the script runs one warm-up sweep, then collects one
 sweep + backtrace (step 0) and prints one JSON line with the share of CTA time in each phase:
 
-    input      staging the tile's input (bulk copies / gather) and transposing it into the local order
+    input      staging the tile's input (bulk copies / gather) and transposing it into the local order (of which
+               `producer_wait`: thread 0 waiting for the producer panel)
     tables     issuing the next tile's prefetch, waiting for the column records (requested when the item started) and
                building the per-column tables
     columns    the column loop (of which `barrier_wait`: thread 0 waiting at the split column barrier)
@@ -37,7 +39,7 @@ CSRC = os.path.join(ROOT, "whatshap_b200", "csrc")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 OBJS = ["whmec.o", "genotype.o", "col_plan.o", "gl_pack.o", "pack.o", "tile_plan.o", "hostpool.o", "readselect.o", "heuristic.o"]
-REC_WORDS = 8  # PhaseRec: t[5], wait, (smid, block), (steady, pad)
+REC_WORDS = 8  # PhaseRec: t[5], wait, (smid, block), (steady, producer_wait)
 CAP = 1 << 20
 
 
@@ -67,6 +69,7 @@ def shares(rec: np.ndarray) -> dict:
     wait = float(rec[:, 5].astype(np.int64).sum())
     out = {name: round(float(d[:, i].sum()) / total, 4) for i, name in enumerate(("input", "tables", "columns", "writeback"))}
     out["barrier_wait"] = round(wait / total, 4)
+    out["producer_wait"] = round(float((rec[:, 7] >> np.uint64(32)).astype(np.int64).sum()) / total, 4)
     out["outside_plus_wait"] = round((float(d[:, 0].sum() + d[:, 1].sum() + d[:, 3].sum()) + wait) / total, 4)
     out["items"] = int(len(rec))
     out["mean_item_cycles"] = round(total / max(len(rec), 1), 1)

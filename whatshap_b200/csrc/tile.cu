@@ -61,9 +61,11 @@ struct TileSmem {
     Panel P;
     uint32_t cg[2];
     uint32_t a_col[TC_CHUNK];
-    uint32_t panel_index;
+    uint32_t first_item, next_item;  // work items claimed by thread 0: the CTA's first, the one after the current
+    uint32_t next_ready;             // the producer of the next item is complete: its input may be prefetched
 #ifdef WHMEC_TILE_PHASE_CLOCKS
     unsigned long long phase_wait;  // thread 0's cycles in the column barrier's wait during the current work item
+    uint32_t phase_pwait;           // ... and waiting for the producer panel's counter
 #endif
 };
 static_assert(sizeof(TileSmem) <= 227 * 1024, "TileSmem exceeds the shared memory of one CTA on sm_90");
@@ -309,7 +311,11 @@ __device__ __forceinline__ bool bulk_handoff(uint32_t gA, uint32_t jb) { return 
 // Bulk version of stage_tile_async (called by warp 0 only): chunk tA lands at stage + tA * (2^j + BULK_SKEW), in the
 // producer's order -- ascending for a computed producer tile, for an uncomputed one (mirrored producer) the chunk of the
 // mirror tile, which holds the wanted entries in DESCENDING order (the reader flips the offset).
+// The proxy fence orders, before the copies (async proxy): the generic reads of the staging buffer by the previous
+// transposition, and the producer's generic stores of the input, which this CTA acquired through the producer's counter.
 __device__ __forceinline__ void stage_tile_bulk(uint32_t *stage, unsigned long long *bar, const Panel *pp, uint32_t ptile, const uint32_t *state) {
+    // (the two state spaces separately: the unqualified fence.proxy.async adds a MEMBAR.GPU)
+    asm volatile("fence.proxy.async.shared::cta;\n fence.proxy.async.global;" ::: "memory");
     const uint32_t gA = __ldg(&pp->in_gA), jb = __ldg(&pp->in_j), sA = __ldg(&pp->in_sA);
     const uint32_t told = ptile & low_mask(__ldg(&pp->in_gold));
     const uint32_t top = __ldg(&pp->in_half) ? (1u << (gA - 1)) : 0u;
@@ -355,7 +361,8 @@ constexpr uint32_t PHASE_CAP = 1u << 20;  // records kept per collection; later 
 struct PhaseRec {
     unsigned long long t[5];
     unsigned long long wait;
-    uint32_t smid, block, steady, pad;
+    uint32_t smid, block, steady;
+    uint32_t producer_wait;  // thread 0's cycles waiting for the producer panel's counter (part of the input phase)
 };
 __device__ PhaseRec g_phase_rec[PHASE_CAP];
 __device__ unsigned int g_phase_n;
@@ -365,38 +372,74 @@ __device__ unsigned int g_phase_n;
 #define WHMEC_PHASE(i)
 #endif
 
+// One launch sweeps one segment: panels [p0, ...) with the work items [item0, item0 + n_items) (a resident sweep: everything).
+struct TileLaunch {
+    uint32_t p0, item0, n_items;
+    int32_t tile_log;              // >= 0: every panel of the segment has 2^tile_log tiles, panel = p0 + ((item - item0) >> tile_log)
+    uint32_t item_lg;              // otherwise panel = item_panel[item >> item_lg] (every panel of the sweep has >= 2^item_lg tiles)
+    const uint32_t *item_panel;
+    uint32_t *done;                // [panel]: tiles of the panel whose write-back is complete (zeroed before the launch)
+    uint32_t *ticket;              // work items of the segment claimed so far (zeroed before the launch)
+};
+
+__device__ __forceinline__ uint32_t panel_of(const TileLaunch &L, uint32_t item) {
+    return L.tile_log >= 0 ? L.p0 + ((item - L.item0) >> L.tile_log) : __ldg(&L.item_panel[item >> L.item_lg]);
+}
+__device__ __forceinline__ uint32_t ld_acquire_gpu(const uint32_t *p) {
+    uint32_t v;
+    asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+    return v;
+}
+__device__ __forceinline__ void red_release_gpu_add(uint32_t *p, uint32_t v) {
+    asm volatile("red.release.gpu.global.add.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
+
+// Schedule of one launch.  Thread 0 of every persistent CTA claims work items with atomicAdd on the launch's ticket, one item
+// ahead (while it sweeps item t it already holds the next one, whose input it prefetches into the staging buffer).  Items are
+// claimed in ascending order and every panel's items come after its producer's, so the launch cannot deadlock, whether or
+// not all its CTAs are resident: the lowest unfinished item is held by a running CTA (tickets only go to running CTAs, and a
+// CTA that holds it as its next item has finished its current, lower one), and all that item's producer tiles have lower
+// tickets, hence are finished.  A static blockIdx + k * gridDim assignment would instead hang as soon as a CTA that owns a
+// producer tile cannot become resident (another stream of the process holding SMs).
+//
+// Completion counters.  A tile of panel r + 1 of a chain reads what all tiles of panel r wrote (canonical hand-off: pdep'ed
+// from everywhere; tile-major: one chunk of every producer tile), so it waits for done[r] == panel_tiles(r): the producer's
+// write-back, bar.sync, then one thread's release add (cumulative: it covers the stores of the whole CTA); the consumer's
+// thread 0 acquires the count, bar.sync, and the warp that issues bulk copies fences the generic -> async proxy.  Fresh
+// panels and producers in an earlier launch (kernel boundary) do not wait.  Panel r + 1 also WRITES the buffer that panel r read (the chain's two state buffers alternate).  That is safe by the same
+// count: every tile of panel r loaded its input into shared memory before it signalled.
 __global__ void __launch_bounds__(NT, 1)
-tile_panel_kernel(const Panel *__restrict__ panels, uint32_t n_panels, uint32_t total_tiles, int32_t tile_log, const TileCol *__restrict__ tcols,
-                  const ColMeta *__restrict__ cols, uint32_t *__restrict__ state, uint32_t *__restrict__ arena,
-                  unsigned long long *__restrict__ chain_keys) {
+tile_panel_kernel(const Panel *__restrict__ panels, const TileLaunch L, const TileCol *__restrict__ tcols, const ColMeta *__restrict__ cols,
+                  uint32_t *state, uint32_t *__restrict__ arena, unsigned long long *__restrict__ chain_keys) {
+    // (`state` is written by other CTAs of the same launch: no __restrict__, so that no load of it becomes a non-coherent one)
     extern __shared__ __align__(16) unsigned char smem_raw[];
     TileSmem &S = *reinterpret_cast<TileSmem *>(smem_raw);
     const uint32_t tid = threadIdx.x;
 
-    // Persistent CTAs: each walks the launch's tiles with stride gridDim.x and, while it sweeps one
-    // tile's panel, the input of its next tile is already streaming into the third buffer (cp.async).
-    uint32_t pi = 0;            // panel of the current work item; panels[] is sorted by tile_begin
     uint32_t staged = 0;        // the staging buffer holds (or is receiving) the current tile's input: 1 = cp.async, 2 = bulk copies
     uint32_t bar_phase = 0;     // parity of the staging mbarrier's current phase
     uint32_t col_phase = 0;     // parity of the column barrier's current phase
     if (tid == 0) {
         mbar_init(&S.stage_bar, 1);
         mbar_init(&S.col_bar, WHMEC_COL_ARRIVE_ALL ? NT : NT / 32);
+        S.first_item = atomicAdd(L.ticket, 1u);
     }
     __syncthreads();
-    for (uint32_t work = blockIdx.x; work < total_tiles; work += gridDim.x) {
+    for (uint32_t t = S.first_item; t < L.n_items;) {
 #ifdef WHMEC_TILE_PHASE_CLOCKS
     unsigned long long ph[5];
     WHMEC_PHASE(0);
-    if (tid == 0) S.phase_wait = 0;
+    if (tid == 0) S.phase_wait = S.phase_pwait = 0;
 #endif
-    if (tile_log >= 0) pi = work >> tile_log;  // every panel of this launch has 2^tile_log tiles
-    else while (pi + 1 < n_panels && __ldg(&panels[pi + 1].tile_begin) <= work) ++pi;
-    __syncthreads();  // previous work item completely done (its stores read the buffers, S.P is reused)
+    const uint32_t work = L.item0 + t;
+    const uint32_t pi = panel_of(L, work);
+    // (the previous work item ended with a barrier: S.P and S.next_item are free)
     if (tid < sizeof(Panel) / 4) ((uint32_t *)&S.P)[tid] = ((const uint32_t *)&panels[pi])[tid];
+    if (tid == 0) S.next_item = atomicAdd(L.ticket, 1u);
     __syncthreads();
     const Panel &P = S.P;
     const uint32_t tile = work - P.tile_begin;
+    const uint32_t tn = S.next_item;
     uint32_t cur = 0;
     // Steady-state panels: their column descriptors start streaming into shared memory now, under the wait for the input.
     if (P.steady) {
@@ -410,15 +453,34 @@ tile_panel_kernel(const Panel *__restrict__ panels, uint32_t n_panels, uint32_t 
     // so that these loads are in flight under the input wait.  next = (panel << 2) | mode, mode 0 = nothing to prefetch,
     // 1 = cp.async gather, 2 = bulk copies.
     uint32_t next = 0;
-    {
-        const uint32_t nwork = work + gridDim.x;
-        if (nwork < total_tiles) {
-            uint32_t pn = pi;
-            if (tile_log >= 0) pn = nwork >> tile_log;
-            else while (pn + 1 < n_panels && __ldg(&panels[pn + 1].tile_begin) <= nwork) ++pn;
-            if (__ldg(&panels[pn].in_layout) == 1 && !__ldg(&panels[pn].fresh))
-                next = (pn << 2) | (bulk_handoff(__ldg(&panels[pn].in_gA), __ldg(&panels[pn].in_j)) ? 2u : 1u);
+    if (tn < L.n_items) {
+        const uint32_t pn = panel_of(L, L.item0 + tn);
+        if (__ldg(&panels[pn].in_layout) == 1 && !__ldg(&panels[pn].fresh))
+            next = (pn << 2) | (bulk_handoff(__ldg(&panels[pn].in_gA), __ldg(&panels[pn].in_j)) ? 2u : 1u);
+    }
+    // The next tile's input is prefetched only if its producer is already complete, checked without blocking (else that
+    // work item fetches its input itself, after waiting).  The last warp checks, so that the loads' latency passes under
+    // this item's input phase instead of in front of the barrier that frees the staging buffer.
+    if (tid == NT - 32 && next) {
+        const Panel *pn = &panels[next >> 2];
+        const uint32_t prod = __ldg(&pn->producer);
+        S.next_ready = prod < L.p0 || ld_acquire_gpu(&L.done[prod]) >= __ldg(&pn->producer_tiles);
+    }
+    // An input that was not prefetched may still be in the making: wait for the producer's counter.
+    if (!staged && !P.fresh && P.producer >= L.p0) {
+        if (tid == 0) {
+#ifdef WHMEC_TILE_PHASE_CLOCKS
+            const long long w0 = clock64();
+#endif
+            for (uint32_t ns = 32; ld_acquire_gpu(&L.done[P.producer]) < P.producer_tiles;) {
+                __nanosleep(ns);
+                if (ns < 1024) ns <<= 1;
+            }
+#ifdef WHMEC_TILE_PHASE_CLOCKS
+            S.phase_pwait = (uint32_t)(clock64() - w0);
+#endif
         }
+        __syncthreads();
     }
 
     // ---- the tile's slice of the incoming projection column
@@ -478,18 +540,15 @@ tile_panel_kernel(const Panel *__restrict__ panels, uint32_t n_panels, uint32_t 
             S.buf[0][l] = src[e];
         }
     }
-    __syncthreads();  // staging buffer free again
+    __syncthreads();  // staging buffer free again (and S.next_ready written)
     WHMEC_PHASE(1);
     // ---- prefetch the input of this CTA's next tile
-    staged = next & 3u;
+    staged = (next && S.next_ready) ? next & 3u : 0u;
     if (staged) {
         const Panel *pn = &panels[next >> 2];
-        const uint32_t ntile = work + gridDim.x - __ldg(&pn->tile_begin);
+        const uint32_t ntile = L.item0 + tn - __ldg(&pn->tile_begin);
         if (staged == 2) {
-            if (tid < 32) {
-                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic reads of the buffer above -> async writes
-                stage_tile_bulk(S.buf[2], &S.stage_bar, pn, ntile, state);
-            }
+            if (tid < 32) stage_tile_bulk(S.buf[2], &S.stage_bar, pn, ntile, state);
         } else {
             stage_tile_async(S.buf[2], pn, ntile, state);
         }
@@ -688,6 +747,14 @@ tile_panel_kernel(const Panel *__restrict__ panels, uint32_t n_panels, uint32_t 
         uint32_t *dst = state + P.out_off;
         for (uint32_t l = tid, it = 0; l < nout; l += NT, ++it) dst[lo | pdep32(it, himask) | gpart] = S.buf[cur][l];
     }
+    const bool produces = !P.ends_chain;
+#ifdef WHMEC_TILE_PHASE_CLOCKS
+    const uint32_t steady = P.steady;
+#endif
+    __syncthreads();  // the tile's write-back is issued by every thread (and S.P, S.next_item are free for the next item)
+    // The release waits until the write-back has reached L2: the last warp signals, while warp 0 already loads the next
+    // item's panel record and claims the item after it.  It signals before this CTA can wait for anything in its next item.
+    if (tid == NT - 32 && produces) red_release_gpu_add(&L.done[pi], 1u);
 #ifdef WHMEC_TILE_PHASE_CLOCKS
     WHMEC_PHASE(4);
     if (tid == 0) {
@@ -700,11 +767,12 @@ tile_panel_kernel(const Panel *__restrict__ panels, uint32_t n_panels, uint32_t 
             asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
             r.smid = smid;
             r.block = blockIdx.x;
-            r.steady = P.steady;
-            r.pad = 0;
+            r.steady = steady;
+            r.producer_wait = S.phase_pwait;
         }
     }
 #endif
+    t = tn;
     }  // work loop
 }
 
@@ -791,11 +859,15 @@ __global__ void __launch_bounds__(32) tile_backtrace_kernel(const ColMeta *__res
 struct TileSeg {
     uint32_t r0, r1;       // rounds [r0, r1)
     uint64_t words;        // back-pointer words of the segment
+    TileLaunch launch;     // its one launch (set by TilePlan::create)
 };
 
 struct TileImpl {
     TileSchedule ts;
     std::vector<TileSeg> segs;          // one segment: everything resident (the usual case)
+    uint32_t *d_sync = nullptr;         // [panel] completion counters, then the ticket of the running launch
+    uint32_t *d_item_panel = nullptr;   // panel of every 2^item_lg work items (only when a segment's panels differ in tiles)
+    std::vector<uint32_t> item_panel;   // its host copy (kept: the upload is asynchronous)
     uint32_t *d_ckpt = nullptr;         // projection state before segments 1 .. K-1 (state_words each)
     uint32_t *d_seg_lo = nullptr, *d_seg_hi = nullptr;  // [segment][chain]: columns of the chain inside the segment (lo > hi: none)
     std::vector<uint32_t> seg_lo, seg_hi;  // their host copies (kept: the upload is asynchronous)
@@ -844,12 +916,28 @@ int TilePlan::create(const Packed &pk, cudaStream_t stream, uint64_t &h2d, std::
     TileSchedule &ts = I->ts;
     I->n_chains = (uint32_t)pk.chain_begin.size() - 1;
     const size_t free_b = device_available_bytes();
+    // Panel look-up of the kernel: a shift where every panel has the same number of tiles, else a table with one entry per
+    // 2^item_lg work items (every tile count is a power of two >= 2^item_lg, so every panel starts on such a boundary)
+    const uint32_t n_panels = (uint32_t)ts.panels.size();
+    uint32_t item_lg = 31, max_lg = 0;
+    for (const Panel &P : ts.panels) {
+        item_lg = std::min(item_lg, P.g - P.half);
+        max_lg = std::max(max_lg, P.g - P.half);
+    }
+    const uint64_t n_items = n_panels ? (uint64_t)ts.panels[n_panels - 1].tile_begin + panel_tiles(ts.panels[n_panels - 1]) : 0;
+    I->item_panel.clear();
+    if (item_lg != max_lg) {
+        I->item_panel.resize(n_items >> item_lg);
+        for (uint32_t q = 0; q < n_panels; ++q)
+            for (uint32_t i = ts.panels[q].tile_begin >> item_lg; i < (ts.panels[q].tile_begin + panel_tiles(ts.panels[q])) >> item_lg; ++i)
+                I->item_panel[i] = q;
+    }
     const uint64_t fixed = (ts.state_words + 2) * 4 + (uint64_t)pk.n * (sizeof(TileCol) + sizeof(ColMeta)) + ts.panels.size() * sizeof(Panel) +
-                           (512ull << 20);
+                           (n_panels + 1 + I->item_panel.size()) * 4 + (512ull << 20);
     // Memory-bounded sweep.  The reference bounds its memory by keeping every sqrt(n)-th column and recomputing
     // (pedigreedptable.cpp:103-134,146-173).  Here the 1-bit back-pointers of ALL columns normally stay resident; when they do
-    // not fit (coverage 25 beyond ~90k columns, coverage 26+), the launch rounds are cut into segments whose back-pointers share
-    // one arena: the forward sweep keeps the projection state in front of every segment (a checkpoint) and the back-pointers of
+    // not fit (coverage 25 beyond ~90k columns, coverage 26+), the rounds are cut into segments (one launch each) whose
+    // back-pointers share one arena: the forward sweep keeps the projection state in front of every segment (a checkpoint) and the back-pointers of
     // the last segment; the backtrace walks the last segment, then re-sweeps the one before from its checkpoint, and so on.
     // The last segment is made as large as fits, so the re-swept fraction is small.  WHMEC_TILE_ARENA_BUDGET (bytes): test hook.
     uint64_t budget = free_b > fixed ? free_b - fixed : 0;
@@ -953,6 +1041,25 @@ int TilePlan::create(const Packed &pk, cudaStream_t stream, uint64_t &h2d, std::
     CUDA_TRY(cudaMallocAsync((void **)&I->d_arena, (I->arena_words + 1) * 4, stream));
     CUDA_TRY(cudaMallocAsync((void **)&I->d_chain_begin, pk.chain_begin.size() * 4, stream));
     CUDA_TRY(cudaMallocAsync((void **)&I->d_chain_keys, (size_t)I->n_chains * 8, stream));
+    CUDA_TRY(cudaMallocAsync((void **)&I->d_sync, ((size_t)n_panels + 1) * 4, stream));
+    if (!I->item_panel.empty()) {
+        CUDA_TRY(cudaMallocAsync((void **)&I->d_item_panel, I->item_panel.size() * 4, stream));
+        CUDA_TRY(cudaMemcpyAsync(I->d_item_panel, I->item_panel.data(), I->item_panel.size() * 4, cudaMemcpyHostToDevice, stream));
+    }
+    for (TileSeg &sg : I->segs) {
+        const uint32_t p0 = ts.round_begin[sg.r0], p1 = ts.round_begin[sg.r1];
+        TileLaunch &L = sg.launch;
+        L.p0 = p0;
+        L.item0 = ts.panels[p0].tile_begin;
+        L.n_items = (p1 < n_panels ? ts.panels[p1].tile_begin : (uint32_t)n_items) - L.item0;
+        bool uniform = true;
+        for (uint32_t q = p0 + 1; q < p1 && uniform; ++q) uniform = ts.panels[q].g - ts.panels[q].half == ts.panels[p0].g - ts.panels[p0].half;
+        L.tile_log = uniform ? (int32_t)(ts.panels[p0].g - ts.panels[p0].half) : -1;
+        L.item_lg = item_lg;
+        L.item_panel = I->d_item_panel;
+        L.done = I->d_sync;
+        L.ticket = I->d_sync + n_panels;
+    }
     const auto tq1 = cclk::now();
     auto up = [&](void *dst, const void *src, size_t bytes) {
         h2d += bytes;
@@ -991,16 +1098,13 @@ int TilePlan::create(const Packed &pk, cudaStream_t stream, uint64_t &h2d, std::
 }
 
 namespace {
-// the launch rounds [r0, r1) of a schedule
-void launch_rounds(TileImpl *I, uint32_t r0, uint32_t r1, cudaStream_t stream, uint32_t &launches) {
-    const TileSchedule &ts = I->ts;
-    for (uint32_t r = r0; r < r1; ++r) {
-        const uint32_t p0 = ts.round_begin[r], p1 = ts.round_begin[r + 1];
-        const uint32_t grid = std::min<uint32_t>(ts.round_tiles[r], I->n_sm);
-        tile_panel_kernel<<<grid, NT, sizeof(TileSmem), stream>>>(I->d_panels + p0, p1 - p0, ts.round_tiles[r], ts.round_tile_log[r], I->d_tcols, I->d_cols,
-                                                                                I->d_state, I->d_arena, I->d_chain_keys);
-        ++launches;
-    }
+// one segment of a schedule: one launch of min(items, SMs) persistent CTAs, its counters and ticket zeroed in front of it
+cudaError_t launch_segment(TileImpl *I, const TileSeg &sg, cudaStream_t stream) {
+    const cudaError_t e = cudaMemsetAsync(I->d_sync, 0, (I->ts.panels.size() + 1) * 4, stream);
+    if (e != cudaSuccess) return e;
+    const uint32_t grid = std::min<uint32_t>(sg.launch.n_items, I->n_sm);
+    tile_panel_kernel<<<grid, NT, sizeof(TileSmem), stream>>>(I->d_panels, sg.launch, I->d_tcols, I->d_cols, I->d_state, I->d_arena, I->d_chain_keys);
+    return cudaGetLastError();
 }
 }  // namespace
 
@@ -1012,9 +1116,9 @@ int TilePlan::sweep(const Packed &pk, cudaStream_t stream, std::string &msg) {
     for (size_t sgi = 0; sgi < I->segs.size(); ++sgi) {
         if (sgi > 0)  // checkpoint: the projection state in front of segment sgi
             CUDA_TRY(cudaMemcpyAsync(I->d_ckpt + (sgi - 1) * (ts.state_words + 1), I->d_state, (ts.state_words + 1) * 4, cudaMemcpyDeviceToDevice, stream));
-        launch_rounds(I, I->segs[sgi].r0, I->segs[sgi].r1, stream, launches);
+        CUDA_TRY(launch_segment(I, I->segs[sgi], stream));
+        ++launches;
     }
-    CUDA_TRY(cudaGetLastError());
     return WHMEC_OK;
 }
 
@@ -1026,9 +1130,8 @@ int TilePlan::backtrace(const Packed &pk, cudaStream_t stream, uint32_t *d_path_
         if (sgi + 1 < I->segs.size()) {  // its back-pointers were overwritten by the later segments: sweep it again from its checkpoint
             if (sgi > 0)
                 CUDA_TRY(cudaMemcpyAsync(I->d_state, I->d_ckpt + (sgi - 1) * (ts.state_words + 1), (ts.state_words + 1) * 4, cudaMemcpyDeviceToDevice, stream));
-            uint32_t again = 0;
-            launch_rounds(I, I->segs[sgi].r0, I->segs[sgi].r1, stream, again);
-            launches += again;
+            CUDA_TRY(launch_segment(I, I->segs[sgi], stream));
+            ++launches;
         }
         tile_backtrace_kernel<<<I->n_chains, 32, 0, stream>>>(I->d_cols, I->d_tcols, I->d_arena, I->d_chain_begin, I->d_seg_lo + sgi * I->n_chains,
                                                               I->d_seg_hi + sgi * I->n_chains, I->n_chains, I->d_chain_keys, d_path_index, d_result);
@@ -1041,7 +1144,8 @@ void TilePlan::release(cudaStream_t stream) {
     TileImpl *I = (TileImpl *)impl;
     if (!I) return;
     for (void *q : {(void *)I->d_tcols, (void *)I->d_panels, (void *)I->d_state, (void *)I->d_arena,
-                    (void *)I->d_chain_begin, (void *)I->d_chain_keys, (void *)I->d_ckpt, (void *)I->d_seg_lo, (void *)I->d_seg_hi})
+                    (void *)I->d_chain_begin, (void *)I->d_chain_keys, (void *)I->d_ckpt, (void *)I->d_seg_lo, (void *)I->d_seg_hi,
+                    (void *)I->d_sync, (void *)I->d_item_panel})
         if (q) cudaFreeAsync(q, stream);
     delete I;
     impl = nullptr;

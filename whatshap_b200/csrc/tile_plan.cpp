@@ -409,32 +409,40 @@ void plan_tiles(const Packed &pk, TileSchedule &ts) {
         }
     });
 
-    // launch rounds: round r = r-th panel of every chain that has one; every round fills its own slice of the panel array
+    // rounds: round r = r-th panel of every chain that has one; every round fills its own slice of the panel array and of the
+    // work-item order
     ts.round_begin.assign(max_panels + 1, 0);
-    for (uint32_t c = 0; c < n_chains; ++c)
-        for (size_t r = 0; r < per_chain[c].size(); ++r) ++ts.round_begin[r + 1];
-    for (size_t r = 0; r < max_panels; ++r) ts.round_begin[r + 1] += ts.round_begin[r];
-    ts.panels.resize(ts.round_begin[max_panels]);
     ts.round_tiles.assign(max_panels, 0);
-    ts.round_tile_log.assign(max_panels, -1);
+    for (uint32_t c = 0; c < n_chains; ++c)
+        for (size_t r = 0; r < per_chain[c].size(); ++r) {
+            ++ts.round_begin[r + 1];
+            ts.round_tiles[r] += panel_tiles(per_chain[c][r]);
+        }
+    std::vector<uint32_t> round_item(max_panels + 1, 0);
+    for (size_t r = 0; r < max_panels; ++r) {
+        ts.round_begin[r + 1] += ts.round_begin[r];
+        round_item[r + 1] = round_item[r] + ts.round_tiles[r];
+    }
+    ts.panels.resize(ts.round_begin[max_panels]);
     parallel_tasks((uint32_t)max_panels, asm_threads, [&](uint32_t r) {
-        uint32_t tiles = 0, at = ts.round_begin[r];
-        int32_t tlog = -1;
-        bool uniform = true;
+        uint32_t item = round_item[r], at = ts.round_begin[r];
         for (uint32_t c = 0; c < n_chains; ++c)
             if (r < per_chain[c].size()) {
-                Panel &P = ts.panels[at];
+                Panel &P = ts.panels[at++];
                 P = per_chain[c][r];
-                P.tile_begin = tiles;
-                tiles += 1u << (P.g - P.half);
-                const int32_t mine = (int32_t)(P.g - P.half);
-                if (at == ts.round_begin[r]) tlog = mine;
-                else if (tlog != mine) uniform = false;
-                ++at;
+                P.tile_begin = item;
+                item += panel_tiles(P);
             }
-        ts.round_tiles[r] = tiles;
-        ts.round_tile_log[r] = (uniform && tlog >= 0) ? tlog : -1;
     });
+    {
+        std::vector<uint32_t> last(n_chains, TILE_NO_PANEL);  // latest panel of every chain so far
+        for (uint32_t q = 0; q < (uint32_t)ts.panels.size(); ++q) {
+            Panel &P = ts.panels[q];
+            P.producer = last[P.chain];
+            P.producer_tiles = P.producer == TILE_NO_PANEL ? 0 : panel_tiles(ts.panels[P.producer]);
+            last[P.chain] = q;
+        }
+    }
     ts.state_words = state_words;
     ts.bp_words = bp_words;
     ts.eligible = true;

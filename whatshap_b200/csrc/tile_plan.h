@@ -61,7 +61,7 @@ struct Panel {
     uint32_t lmask_out, gmask_out; // canonical masks over the output state's bits (unused if ends_chain)
     uint32_t ends_chain;           // last column is the chain end: no state is written
     uint32_t fresh;                // first panel of its chain: the input state is the single value 0
-    uint32_t tile_begin;           // first CTA of this panel inside its launch
+    uint32_t tile_begin;           // first work item (one tile of one panel) of this panel in the sweep's item order
     // State hand-off layout between consecutive panels of a chain.  0 = canonical (the reference's
     // forward-projection index).  1 = tile-major: the producer tile t writes its 2^s_out entries
     // contiguously at (t << s_out); possible when the consumer's local reads are the producer's
@@ -83,17 +83,25 @@ struct Panel {
     // back-pointers, one mirror mode.  The kernel sweeps such a panel with all per-column tables built once, in
     // parallel, and no per-column dispatch.  steady = 1 + LG (2^LG twin pairs per thread), 0 otherwise.
     uint32_t steady;
+    // The previous panel of the chain (index into TileSchedule::panels; TILE_NO_PANEL for a fresh panel), whose output is this
+    // panel's input, and its number of computed tiles: the kernel starts a tile of this panel once that many tiles of the
+    // producer have signalled their write-back.
+    uint32_t producer, producer_tiles;
     uint64_t in_off, out_off;      // 32-bit word offsets of the chain's state buffers
 };
+constexpr uint32_t TILE_NO_PANEL = 0xFFFFFFFFu;
+inline uint32_t panel_tiles(const Panel &P) { return 1u << (P.g - P.half); }  // computed tiles (mirrored panel: half of 2^g)
 
 struct TileSchedule {
     bool eligible = false;
     std::string why;                      // reason when not eligible
     StagedVec<TileCol> cols;              // [n] indexed by global column (uploaded as it is)
-    StagedVec<Panel> panels;              // grouped by launch round (uploaded as it is)
+    // Round r = the r-th panel of every chain that has one.  panels[] is grouped round by round (chains ascending inside a
+    // round) and its work items are numbered in that order, so a panel's producer always comes earlier; segments of a
+    // memory-bounded sweep are cut at round boundaries.
+    StagedVec<Panel> panels;              // (uploaded as it is)
     std::vector<uint32_t> round_begin;    // panels of round r: [round_begin[r], round_begin[r+1])
-    std::vector<uint32_t> round_tiles;    // CTAs per round
-    std::vector<int32_t> round_tile_log;  // log2 tiles per panel if every panel of the round has the same number, else -1
+    std::vector<uint32_t> round_tiles;    // work items of round r
     uint64_t state_words = 0;             // total size of the per-chain state double buffers
     uint64_t bp_words = 0;
     uint64_t state_traffic_bytes = 0;     // bytes of state written + read through global memory
