@@ -130,6 +130,32 @@ void whmec_plan_destroy(whmec_plan *plan);
 int whmec_solve(const whmec_problem *p, whmec_solution *s, int device, whmec_stats *st_or_null,
                 char *err, size_t errlen);
 
+/* ---- Several tables in one call --------------------------------------------------------------------------
+ * `whatshap phase` builds one PedigreeDPTable per (chromosome x family); one such table rarely fills a GPU.  This entry point
+ * takes n_tables independent problems and gives every one of them the solution whmec_solve gives it alone, bit for bit
+ * (cost, path, partition, super-reads, ties included).
+ *   - Single-individual tables that the tile kernel covers are swept TOGETHER: their chains are as independent as the chains
+ *     of one table, so one persistent launch sweeps the panels of all of them, one launch backtraces all chains, and the
+ *     per-table costs are reduced on the device.  Tables are grouped (consecutively) so that a group's device memory fits
+ *     under one reading of the free memory; a table that does not fit alone takes the single-table path.
+ *   - Trio tables (T = 4) whose columns all have the fused kernel's shape are swept TOGETHER as well: pass 1 and pass 2 of the
+ *     fused sweep take the union of their chains, the fold between the passes restarts at every table, and the backtrace
+ *     enters every table's last chain at that table's optimum.  Groups are cut under WHMEC_COLUMN_ARENA_BUDGET likewise.
+ *   - Every other table (larger pedigrees, distrusted genotypes outside the fused shape, tables the tile planner declines,
+ *     tables without columns) is solved inside the call by the single-table path, one after the other.
+ * Errors are per table: status[t] and the message at errs + t * errlen (errs may be NULL) are what whmec_solve would have
+ * returned for table t -- a Mendelian conflict or unsorted input in one table leaves the others solved.  The return value is
+ * WHMEC_OK unless the call itself failed: WHMEC_ERR_INPUT for null arguments, WHMEC_ERR_CUDA for a CUDA failure (then every
+ * status[] holds the code and every message the reason; running out of host memory fails the call the same way, with
+ * WHMEC_ERR_UNSUPPORTED).  n_tables == 0 does nothing.  Every table of the list is packed on the host before the first sweep:
+ * hand long lists over in slices.
+ * stats (optional, [n_tables]): cells, algorithmic bytes, chains, max_active, T, path_kind, back-pointer and state bytes of
+ * every table; times are 0 (tables share their sweeps).  total (optional): sums over the call; sweep_ms is the device time of
+ * all sweeps, kernel_launches counts the sweep launches of the whole call, path_kind is 0 when the tables took different paths. */
+int whmec_solve_batch(const whmec_problem *const *problems, whmec_solution *const *solutions, uint32_t n_tables, int device,
+                      int *status /* [n_tables] */, char *errs /* [n_tables][errlen] or NULL */, size_t errlen,
+                      whmec_stats *stats_or_null /* [n_tables] */, whmec_stats *total_or_null);
+
 /* ---- Genotype likelihoods by the forward-backward algorithm (the reference's GenotypeDPTable) ----------
  * Same inputs as whmec_solve, read differently where the reference does: p->gl holds, per individual and
  * column, the PRIOR probabilities of the genotypes 0/0, 0/1, 1/1 (required; the reference asserts on missing

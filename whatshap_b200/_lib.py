@@ -9,7 +9,7 @@ import ctypes as C
 import os
 import subprocess
 from functools import lru_cache
-from typing import Optional, Tuple
+from typing import List, Optional, Sequence, Tuple, Union
 
 import numpy as np
 
@@ -29,6 +29,7 @@ EXPORTS = (
     "whmec_plan_stats",
     "whmec_plan_destroy",
     "whmec_solve",
+    "whmec_solve_batch",
     "whmec_segment_create",
     "whmec_segment_transfer",
     "whmec_segment_sweep",
@@ -77,6 +78,9 @@ def lib() -> C.CDLL:
     L.whmec_plan_destroy.argtypes = [C.c_void_p]
     L.whmec_plan_destroy.restype = None
     L.whmec_solve.argtypes = [C.POINTER(CProblem), C.POINTER(CSolution), C.c_int, C.POINTER(CStats), C.c_char_p, C.c_size_t]
+    L.whmec_solve_batch.argtypes = [C.POINTER(C.POINTER(CProblem)), C.POINTER(C.POINTER(CSolution)), C.c_uint32, C.c_int, C.POINTER(C.c_int),
+                                    C.c_char_p, C.c_size_t, C.POINTER(CStats), C.POINTER(CStats)]
+    L.whmec_solve_batch.restype = C.c_int
     L.whmec_genotype.argtypes = [C.POINTER(CProblem), C.POINTER(C.c_double), C.c_int, C.POINTER(CStats), C.c_char_p, C.c_size_t]
     L.whmec_genotype.restype = C.c_int
     L.whmec_compute_genotypes.argtypes = [C.POINTER(CProblem), C.POINTER(C.c_double), C.POINTER(C.c_int8), C.c_char_p, C.c_size_t]
@@ -133,6 +137,36 @@ def solve(prob: FlatProblem, device: int = 0) -> Tuple[FlatSolution, dict]:
     raise_for(rc, err.value.decode())
     sol.cost = int(cs.cost)
     return sol, st.as_dict()
+
+
+def solve_batch(problems: Sequence[FlatProblem], device: int = 0, with_stats: bool = False):
+    """Several tables through one `whmec_solve_batch`: a list with, per table and in input order, its `FlatSolution` -- bit for
+    bit what `solve` gives for it alone -- or the exception `solve` would have raised for it (the other tables are still solved).
+    A failure of the call itself (no device, a CUDA error) raises.  `with_stats`: also returns (per-table stats, totals of the call)."""
+    n = len(problems)
+    sols = [FlatSolution(p.n_cols, p.n_reads, p.n_ind) for p in problems]
+    cps, css = [p.as_c() for p in problems], [s.as_c() for s in sols]
+    pp = (C.POINTER(CProblem) * max(n, 1))(*[C.pointer(c) for c in cps])
+    sp = (C.POINTER(CSolution) * max(n, 1))(*[C.pointer(c) for c in css])
+    status = (C.c_int * max(n, 1))()
+    errlen = 512
+    errs = C.create_string_buffer(errlen * max(n, 1))
+    stats, total = (CStats * max(n, 1))(), CStats()
+    rc = lib().whmec_solve_batch(pp, sp, n, device, status, errs, errlen, stats, C.byref(total))
+    messages = [errs.raw[t * errlen:(t + 1) * errlen].split(b"\0", 1)[0].decode() for t in range(n)]
+    if rc != 0:
+        raise_for(rc, messages[0] if messages else "whmec_solve_batch: invalid arguments")
+    out: List[Union[FlatSolution, Exception]] = []
+    for t in range(n):
+        try:
+            raise_for(int(status[t]), messages[t])
+            sols[t].cost = int(css[t].cost)
+            out.append(sols[t])
+        except Exception as e:  # noqa: BLE001 - handed to the caller in the table's place
+            out.append(e)
+    if with_stats:
+        return out, ([stats[t].as_dict() for t in range(n)], total.as_dict())
+    return out
 
 
 def genotype(prob: FlatProblem, device: int = 0) -> Tuple[np.ndarray, dict]:

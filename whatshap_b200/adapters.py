@@ -218,6 +218,38 @@ def make_dp_table_class(core_module, solver=None):
             solve = solver or (lambda p: multigpu.solve_table(p)[0])
             self._solution = solve(self._problem)
 
+        @classmethod
+        def batch(cls, tables, device=0, devices=None, return_exceptions=False):
+            """Several tables in one call (`core.PedigreeDPTable.batch`): `tables` holds constructor argument tuples."""
+            objs = []
+            for args in tables:
+                try:
+                    obj = cls.__new__(cls)
+                    obj.pedigree = args[2]
+                    obj._problem, obj._ids = flatten_objects(args[0], args[1], args[2], args[3] if len(args) > 3 else False,
+                                                             args[4] if len(args) > 4 else None)
+                    objs.append(obj)
+                except Exception as e:  # noqa: BLE001 - reported in the table's place, after the others ran
+                    objs.append(e)
+            good = [i for i, o in enumerate(objs) if not isinstance(o, BaseException)]
+            problems = [objs[i]._problem for i in good]
+            if solver:
+                solutions = []
+                for p in problems:
+                    try:
+                        solutions.append(solver(p))
+                    except Exception as e:  # noqa: BLE001
+                        solutions.append(e)
+            else:
+                solutions = multigpu.solve_tables(problems, device, devices)
+            for i, sol in zip(good, solutions):
+                if isinstance(sol, BaseException):
+                    objs[i] = sol
+                else:
+                    objs[i]._solution = sol
+            multigpu.finish_batch(objs, return_exceptions)
+            return objs
+
         def get_super_reads(self):
             prob, sol = self._problem, self._solution
             positions = prob.positions.tolist()

@@ -755,6 +755,38 @@ class PedigreeDPTable:
         self._problem = _flatten(readset, recombcost, pedigree, bool(distrust_genotypes), positions)
         self._solution, self.stats = multigpu.solve_table(self._problem, device, devices)
 
+    @classmethod
+    def batch(cls, tables, device: int = 0, devices=None, return_exceptions: bool = False) -> list:
+        """Several tables in one call, sharing the GPU (`multigpu.solve_tables`, `whmec_solve_batch`).  `tables` is a sequence of
+        constructor argument tuples `(readset, recombcost, pedigree[, distrust_genotypes[, positions]])`; every returned object
+        behaves exactly like `cls(*arguments)`.  A table that fails does not stop the others: afterwards the error of the
+        lowest-index failing table is raised, with the type and text the constructor would have raised; with
+        `return_exceptions` the exception instance takes the table's place instead."""
+        objs: list = []
+        for args in tables:
+            try:
+                readset, recombcost, pedigree = args[0], args[1], args[2]
+                if not isinstance(readset, ReadSet):
+                    raise TypeError("Argument 'readset' has incorrect type")
+                if not isinstance(pedigree, Pedigree):
+                    raise TypeError("Argument 'pedigree' has incorrect type")
+                obj = cls.__new__(cls)
+                obj.pedigree = pedigree
+                obj._problem = _flatten(readset, recombcost, pedigree, bool(args[3]) if len(args) > 3 else False, args[4] if len(args) > 4 else None)
+                obj.stats = {}
+                objs.append(obj)
+            except Exception as e:  # noqa: BLE001 - reported in the table's place, after the others ran
+                objs.append(e)
+        good = [i for i, o in enumerate(objs) if not isinstance(o, BaseException)]
+        solutions, stats = multigpu.solve_tables([objs[i]._problem for i in good], device, devices, with_stats=True)
+        for i, sol, st in zip(good, solutions, stats):
+            if isinstance(sol, BaseException):
+                objs[i] = sol
+            else:
+                objs[i]._solution, objs[i].stats = sol, st  # (times are 0: the tables shared their sweeps)
+        multigpu.finish_batch(objs, return_exceptions)
+        return objs
+
     def get_super_reads(self) -> Tuple[List[ReadSet], List[int]]:
         """One ReadSet per individual (pedigree order) holding `superread_0_<k>` and
         `superread_1_<k>`, plus the transmission vector (src/pedigreedptable.cpp:344-388)."""

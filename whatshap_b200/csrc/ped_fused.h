@@ -223,6 +223,33 @@ WHMEC_HD void pf_first_row(const ColMeta &m, const uint32_t *invec /* [4], UMAX 
 }
 
 // lanes per projection entry: columns with fewer than PF_THREADS entries spread an entry's 2^d candidates over 2^lc items
+// Pass 1 -> pass 2 for ONE table that starts at chain 0 of `rows` (several tables in one sweep: one thread per table, each on
+// its own chains).  Chain c's transfer matrix is Mat[u][i] = rows[c][i ^ u]; the table's first chain ignores its input (its
+// row IS its output, its input vector is written as zeros); every later chain's true input is the min-plus fold of the
+// chains in front of it -- of THIS table only: the fold restarts where a table starts.
+WHMEC_HD void pf_fold_table(const uint32_t *rows, uint32_t n_chains, uint32_t *in_vecs) {
+    uint32_t in[PF_T], out[PF_T];
+    for (uint32_t i = 0; i < PF_T; ++i) {
+        in[i] = rows[i];
+        in_vecs[i] = 0;
+    }
+    for (uint32_t c = 1; c < n_chains; ++c) {
+        for (uint32_t i = 0; i < PF_T; ++i) {
+            in_vecs[(size_t)c * PF_T + i] = in[i];
+            out[i] = UMAX;
+        }
+        const uint32_t *row = rows + (size_t)c * PF_T;
+        for (uint32_t u = 0; u < PF_T; ++u) {
+            if (in[u] == UMAX) continue;
+            for (uint32_t i = 0; i < PF_T; ++i) {
+                const uint32_t mv = row[i ^ u];
+                if (mv != UMAX && in[u] + mv < out[i]) out[i] = in[u] + mv;
+            }
+        }
+        for (uint32_t i = 0; i < PF_T; ++i) in[i] = out[i];
+    }
+}
+
 WHMEC_HD uint32_t pf_lane_bits(uint32_t f, uint32_t d) {
     uint32_t lc = 0;
     while (((1u << f) << lc) < PF_THREADS && lc < d) ++lc;

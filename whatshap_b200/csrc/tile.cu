@@ -856,6 +856,19 @@ __global__ void __launch_bounds__(32) tile_backtrace_kernel(const ColMeta *__res
     }
 }
 
+// Several tables swept as one union of chains: one warp per table adds up the optima of the table's chains (the cost of a
+// single-individual table is the sum over its DP-independent chains), so that only one word per table travels back.
+__global__ void __launch_bounds__(32) tile_table_cost_kernel(const unsigned long long *__restrict__ chain_keys,
+                                                             const uint32_t *__restrict__ table_chain, uint32_t n_tables,
+                                                             uint32_t *__restrict__ costs) {
+    const uint32_t t = blockIdx.x, lane = threadIdx.x;
+    if (t >= n_tables) return;
+    uint32_t sum = 0;
+    for (uint32_t c = table_chain[t] + lane; c < table_chain[t + 1]; c += 32) sum += (uint32_t)(chain_keys[c] >> 32);
+    for (int off = 16; off > 0; off >>= 1) sum += __shfl_xor_sync(0xFFFFFFFFu, sum, off);
+    if (lane == 0) costs[t] = sum;
+}
+
 struct TileSeg {
     uint32_t r0, r1;       // rounds [r0, r1)
     uint64_t words;        // back-pointer words of the segment
@@ -909,6 +922,14 @@ bool TilePlan::plan(const Packed &pk) {
     backptr_bytes = I->ts.bp_words * 4;
     state_bytes = I->ts.state_traffic_bytes;
     return true;
+}
+
+void TilePlan::adopt(TileSchedule &&ts) {
+    TileImpl *I = new TileImpl();
+    I->ts = std::move(ts);
+    impl = I;
+    backptr_bytes = I->ts.bp_words * 4;
+    state_bytes = I->ts.state_traffic_bytes;
 }
 
 int TilePlan::create(const Packed &pk, cudaStream_t stream, uint64_t &h2d, std::string &msg, const ColMeta *d_cols) {
@@ -1136,6 +1157,13 @@ int TilePlan::backtrace(const Packed &pk, cudaStream_t stream, uint32_t *d_path_
         tile_backtrace_kernel<<<I->n_chains, 32, 0, stream>>>(I->d_cols, I->d_tcols, I->d_arena, I->d_chain_begin, I->d_seg_lo + sgi * I->n_chains,
                                                               I->d_seg_hi + sgi * I->n_chains, I->n_chains, I->d_chain_keys, d_path_index, d_result);
     }
+    CUDA_TRY(cudaGetLastError());
+    return WHMEC_OK;
+}
+
+int TilePlan::table_costs(cudaStream_t stream, const uint32_t *d_table_chain, uint32_t n_tables, uint32_t *d_costs, std::string &msg) {
+    TileImpl *I = (TileImpl *)impl;
+    tile_table_cost_kernel<<<n_tables, 32, 0, stream>>>(I->d_chain_keys, d_table_chain, n_tables, d_costs);
     CUDA_TRY(cudaGetLastError());
     return WHMEC_OK;
 }

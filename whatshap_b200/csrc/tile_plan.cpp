@@ -449,4 +449,110 @@ void plan_tiles(const Packed &pk, TileSchedule &ts) {
     if (timing) std::fprintf(stderr, "[whmec] plan: chains %.2f ms, assemble %.2f ms\n", tms(t0, t1), tms(t1, tnow()));
 }
 
+void merge_tile_tables(const std::vector<const Packed *> &pks, const std::vector<const TileSchedule *> &tss, TileUnion &out) {
+    const size_t B = pks.size();
+    out = TileUnion();
+    TileSchedule &ts = out.ts;
+    out.table_chain.assign(B + 1, 0);
+    out.table_col.assign(B + 1, 0);
+    std::vector<uint64_t> state_base(B + 1, 0), bp_base(B + 1, 0);
+    size_t n_panels = 0, rounds = 0;
+    for (size_t t = 0; t < B; ++t) {
+        out.table_chain[t + 1] = out.table_chain[t] + (uint32_t)pks[t]->chain_begin.size() - 1;
+        out.table_col[t + 1] = out.table_col[t] + pks[t]->n;
+        state_base[t + 1] = state_base[t] + tss[t]->state_words;
+        bp_base[t + 1] = bp_base[t] + tss[t]->bp_words;
+        ts.state_traffic_bytes += tss[t]->state_traffic_bytes;
+        n_panels += tss[t]->panels.size();
+        rounds = std::max(rounds, tss[t]->round_tiles.size());
+    }
+    Packed &pk = out.pk;
+    pk.n = out.table_col[B];
+    pk.cols.resize(pk.n);
+    ts.cols.resize(pk.n);
+    pk.chain_begin.resize((size_t)out.table_chain[B] + 1);
+    parallel_tasks((uint32_t)B, std::min<uint32_t>(host_threads(32), (uint32_t)B), [&](uint32_t t) {
+        const uint32_t k0 = out.table_col[t], n = pks[t]->n;
+        if (n) std::memcpy(&pk.cols[k0], pks[t]->cols.data(), (size_t)n * sizeof(ColMeta));
+        for (uint32_t k = 0; k < n; ++k) {
+            TileCol &tc = ts.cols[k0 + k];
+            tc = tss[t]->cols[k];
+            tc.bp_off += bp_base[t];
+        }
+        for (uint32_t c = out.table_chain[t]; c < out.table_chain[t + 1]; ++c) pk.chain_begin[c] = k0 + pks[t]->chain_begin[c - out.table_chain[t]];
+    });
+    pk.chain_begin[out.table_chain[B]] = pk.n;
+    // rounds of the union; panel_at[t][q] = where panel q of table t went
+    ts.panels.resize(n_panels);
+    ts.round_begin.assign(rounds + 1, 0);
+    ts.round_tiles.assign(rounds, 0);
+    std::vector<std::vector<uint32_t>> panel_at(B);
+    for (size_t t = 0; t < B; ++t) panel_at[t].resize(tss[t]->panels.size());
+    uint32_t at = 0, item = 0;
+    for (size_t r = 0; r < rounds; ++r) {
+        ts.round_begin[r] = at;
+        for (size_t t = 0; t < B; ++t) {
+            if (r >= tss[t]->round_tiles.size()) continue;
+            for (uint32_t q = tss[t]->round_begin[r]; q < tss[t]->round_begin[r + 1]; ++q) {
+                Panel &P = ts.panels[at];
+                P = tss[t]->panels[q];
+                P.chain += out.table_chain[t];
+                P.col_begin += out.table_col[t];
+                P.col_end += out.table_col[t];
+                P.in_off += state_base[t];
+                P.out_off += state_base[t];
+                P.tile_begin = item;
+                if (P.producer != TILE_NO_PANEL) P.producer = panel_at[t][P.producer];
+                panel_at[t][q] = at++;
+                item += panel_tiles(P);
+                ts.round_tiles[r] += panel_tiles(P);
+            }
+        }
+    }
+    ts.round_begin[rounds] = at;
+    ts.state_words = state_base[B];
+    ts.bp_words = bp_base[B];
+    ts.eligible = true;
+}
+
+uint64_t tile_table_items(const TileSchedule &ts) {
+    uint64_t items = 0;
+    for (uint32_t t : ts.round_tiles) items += t;
+    return items;
+}
+
+uint64_t tile_table_bytes(const Packed &pk, const TileSchedule &ts) {
+    const uint64_t chains = pk.chain_begin.size();
+    return (ts.state_words + ts.bp_words + 4) * 4 + (uint64_t)pk.n * (sizeof(TileCol) + sizeof(ColMeta) + 8) +
+           ts.panels.size() * (sizeof(Panel) + 4) + tile_table_items(ts) * 4 + chains * 24;
+}
+
+void cut_table_groups(const std::vector<uint64_t> &bytes, const std::vector<uint64_t> &items, uint64_t budget,
+                      std::vector<std::pair<uint32_t, uint32_t>> &groups, std::vector<uint32_t> &alone) {
+    constexpr uint64_t ITEM_CAP = 1ull << 31;
+    groups.clear();
+    alone.clear();
+    uint32_t first = 0;
+    uint64_t sum_b = 0, sum_i = 0;
+    auto close = [&](uint32_t end) {
+        if (end > first) groups.push_back({first, end});
+        sum_b = sum_i = 0;
+    };
+    for (uint32_t t = 0; t < (uint32_t)bytes.size(); ++t) {
+        if (bytes[t] > budget || items[t] >= ITEM_CAP) {
+            close(t);
+            alone.push_back(t);
+            first = t + 1;
+            continue;
+        }
+        if (sum_b + bytes[t] > budget || sum_i + items[t] >= ITEM_CAP) {
+            close(t);
+            first = t;
+        }
+        sum_b += bytes[t];
+        sum_i += items[t];
+    }
+    close((uint32_t)bytes.size());
+}
+
 }  // namespace whmec

@@ -14,6 +14,7 @@
 #pragma once
 #include <stdint.h>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "pack.h"
@@ -109,5 +110,28 @@ struct TileSchedule {
 
 // Builds the schedule; `eligible == false` (with `why`) means the column kernel must be used.
 void plan_tiles(const Packed &pk, TileSchedule &out);
+
+// ---- several tables in one sweep (whmec_solve_batch) -------------------------------------------------------------------
+// Chains of different single-individual tables are as independent as the chains of one table, so the schedules of several
+// tables concatenate into one: chains, columns, panels, work items, state buffers and back-pointer words are renumbered
+// globally.  Round r of the union is round r of every table that has one (tables in input order), so a panel's producer
+// still comes earlier in the item order and segments can still be cut at round boundaries.
+struct TileUnion {
+    Packed pk;                          // what the sweep and the backtrace read of a packed problem: n, cols, chain_begin
+    TileSchedule ts;
+    std::vector<uint32_t> table_chain;  // [tables + 1] first chain of every table
+    std::vector<uint32_t> table_col;    // [tables + 1] first column of every table
+};
+void merge_tile_tables(const std::vector<const Packed *> &pks, const std::vector<const TileSchedule *> &tss, TileUnion &out);
+
+// Device bytes one table adds to a union (records, state buffers, back-pointers, path) and its work items.
+uint64_t tile_table_bytes(const Packed &pk, const TileSchedule &ts);
+uint64_t tile_table_items(const TileSchedule &ts);
+
+// Cuts tables 0 .. n-1 into consecutive groups [first, last) whose bytes fit `budget` together (and whose `items` -- work items of a
+// tile union, cost functions of a pedigree union: both are numbered in 32 bits -- stay below 2^31); a table that does not fit alone is listed in `alone` instead (it takes the single-table path,
+// which knows the memory-bounded sweep).  One budget for all groups: groups are resident one after the other.
+void cut_table_groups(const std::vector<uint64_t> &bytes, const std::vector<uint64_t> &items, uint64_t budget,
+                      std::vector<std::pair<uint32_t, uint32_t>> &groups, std::vector<uint32_t> &alone);
 
 }  // namespace whmec

@@ -21,10 +21,12 @@
 #include <new>
 #include <stdexcept>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "../../include/whmec.h"
 #include "col_plan.h"
+#include "batch.h"
 #include "common.h"
 #include "dp_device.h"
 #include "ped_fused.h"
@@ -667,6 +669,16 @@ __global__ void ped_fused_prefix_kernel(const uint32_t *__restrict__ rows, uint3
         for (uint32_t i = 0; i < PF_T; ++i) matrix[(size_t)u0 * PF_T + i] = in[i];
 }
 
+// Several trio tables in one fused sweep: thread t folds the chains of table t alone (pf_fold_table), so the fold restarts
+// at every chain that starts a table, exactly as ped_fused_prefix_kernel starts it at chain 0 of a table that does not continue.
+__global__ void ped_fused_tables_prefix_kernel(const uint32_t *__restrict__ rows, const uint32_t *__restrict__ table_chain, uint32_t n_tables,
+                                               uint32_t *__restrict__ in_vecs) {
+    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= n_tables) return;
+    const uint32_t c0 = table_chain[t], c1 = table_chain[t + 1];
+    if (c1 > c0) pf_fold_table(rows + (size_t)c0 * PF_T, c1 - c0, in_vecs + (size_t)c0 * PF_T);
+}
+
 // pass 1 -> pass 2: the T x T transfer matrices of the chains, folded left to right in min-plus
 // arithmetic (a few hundred operations per row).
 //   pass-1 planes: chain c, unit vector u -> slot c*T + u;  pass-2 slot of chain c: n_chains*T + c.
@@ -859,13 +871,17 @@ struct BtArgs {
     const uint32_t *arena, *chain_begin, *last_vals;
     uint32_t T, tb, n_chains;
     int entry;  // prev_tv handed to the last chain by the columns after the plan; < 0: the plan ends the table
+    // several tables in one sweep: table_end[c] = t + 1 when chain c is the last chain of table t (else 0), and last_vals holds
+    // the T final values of EVERY chain; nullptr: one table, which ends with the last chain
+    const uint32_t *table_end;
 };
 
 __device__ __forceinline__ void bt_chain_start(const BtArgs &a, const BtView &bv, uint32_t c, uint32_t u, uint32_t *x,
                                                uint32_t *tv, uint32_t *ptv, uint32_t *cost) {
     const uint32_t k_last = a.chain_begin[c + 1] - 1;
-    if (c + 1 == a.n_chains && a.entry < 0) {
-        pick_optimum(a.cols[k_last], a.last_vals, a.arena, a.T, a.tb, cost, x, tv, ptv);
+    const bool ends_table = a.table_end ? a.table_end[c] != 0 : c + 1 == a.n_chains;
+    if (ends_table && a.entry < 0) {
+        pick_optimum(a.cols[k_last], a.table_end ? a.last_vals + (size_t)c * a.T : a.last_vals, a.arena, a.T, a.tb, cost, x, tv, ptv);
     } else {
         *tv = u;
         chain_entry(bv, k_last, u, x, ptv);
@@ -960,7 +976,24 @@ __global__ void __launch_bounds__(32) bt_paths_kernel(const BtArgs a, const uint
     uint32_t x, tv, ptv, cost = 0;
     bt_chain_start(a, bv, c, entries[c], &x, &tv, &ptv, &cost);
     backtrace_range_warp(bv, S, a.chain_begin[c + 1] - 1, a.chain_begin[c], x, tv, ptv, path_index, path_tv);
-    if (result && c + 1 == a.n_chains && threadIdx.x == 0) result[0] = cost;
+    if (a.table_end) {  // result[t] = cost of table t, from the table's last chain
+        if (result && a.table_end[c] && threadIdx.x == 0) result[a.table_end[c] - 1] = cost;
+    } else if (result && c + 1 == a.n_chains && threadIdx.x == 0) {
+        result[0] = cost;
+    }
+}
+
+// Several tables in one sweep: thread t enters table t's last chain at that table's optimum (whose exit is stored for every
+// entry value alike) and follows the realised entries through the table's chains, right to left.
+__global__ void bt_table_entries_kernel(const BtArgs a, const uint32_t *__restrict__ exits, const uint32_t *__restrict__ table_chain,
+                                        uint32_t n_tables, uint32_t *__restrict__ entries) {
+    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= n_tables) return;
+    uint32_t e = 0;
+    for (uint32_t c = table_chain[t + 1]; c-- > table_chain[t];) {
+        entries[c] = e;
+        e = exits[c * a.T + e];
+    }
 }
 
 // Memory-bounded sequential sweep: one warp walks the columns [k_lo, k_hi] of one segment, whose back-pointers are in the arena
@@ -1225,6 +1258,8 @@ struct whmec_plan {
     DevBuf<uint32_t> d_ckpt, d_bt_state;
     // tile path
     TilePlan tiles;
+    // several tables in one tile sweep (whmec_solve_batch): first chain of every table, cost of every table
+    DevBuf<uint32_t> d_table_chain, d_table_cost, d_table_end;
 
     ~whmec_plan() {
         cudaSetDevice(device);
@@ -1237,7 +1272,7 @@ struct whmec_plan {
         d_ped_steps.release(); d_ped_vals.release(); d_chain_len.release(); d_ped_args.release();
         d_in_vec.release(); d_matrix.release(); d_bt_exits.release(); d_bt_entries.release();
         d_chain_rows.release(); d_chain_in.release(); d_chain_out.release();
-        d_ckpt.release(); d_bt_state.release();
+        d_ckpt.release(); d_bt_state.release(); d_table_chain.release(); d_table_cost.release(); d_table_end.release();
         tiles.release(stream);
         if (graph_exec) cudaGraphExecDestroy(graph_exec);
         StreamSet set{stream, ev0, ev1, evh0, evh1};
@@ -1338,6 +1373,21 @@ int col_create(whmec_plan *pl, bool bounded_t1, uint64_t &h2d, std::string &msg)
     return WHMEC_OK;
 }
 
+// device, stream + events (reused across plans), start of the upload window
+int plan_device_setup(whmec_plan *pl, int device, std::string &msg) {
+    CUDA_TRY(cudaSetDevice(device));
+    keep_pool_memory(device);
+    StreamSet set;
+    CUDA_TRY(g_streams.acquire(device, set));
+    pl->stream = set.stream;
+    pl->ev0 = set.ev0;
+    pl->ev1 = set.ev1;
+    pl->evh0 = set.evh0;
+    pl->evh1 = set.evh1;
+    CUDA_TRY(cudaEventRecord(pl->evh0, pl->stream));
+    return WHMEC_OK;
+}
+
 // bounded_t1: a single individual whose back-pointers exceed the free HBM takes the memory-bounded sweep (solve_impl, once no
 // group of chains fits) instead of being refused
 int plan_create_impl(const whmec_problem *p, int device, whmec_plan *pl, std::string &msg, int segment = 0, bool bounded_t1 = false) {
@@ -1365,19 +1415,7 @@ int plan_create_impl(const whmec_problem *p, int device, whmec_plan *pl, std::st
     Packed &pk = pl->pk;
     const auto tc1 = pclk::now();
     uint64_t h2d = 0;
-    auto device_setup = [&]() -> int {  // device, stream + events (reused across plans), start of the upload window
-        CUDA_TRY(cudaSetDevice(device));
-        keep_pool_memory(device);
-        StreamSet set;
-        CUDA_TRY(g_streams.acquire(device, set));
-        pl->stream = set.stream;
-        pl->ev0 = set.ev0;
-        pl->ev1 = set.ev1;
-        pl->evh0 = set.evh0;
-        pl->evh1 = set.evh1;
-        CUDA_TRY(cudaEventRecord(pl->evh0, pl->stream));
-        return WHMEC_OK;
-    };
+    auto device_setup = [&]() -> int { return plan_device_setup(pl, device, msg); };
     if (tile_candidate && pk.n > 0) {
         // the per-column records of the packer (4 MB for 50k columns) travel while the host plans the tiles
         rc = device_setup();
@@ -1710,7 +1748,7 @@ int plan_sweep_impl(whmec_plan *pl, std::string &msg, bool wait = true) {
 BtArgs bt_args(const whmec_plan *pl, int entry) {
     const Packed &pk = pl->pk;
     return BtArgs{pl->d_cols.p, pl->d_arena.p, pl->d_chain_begin.p, pl->col.two_pass() ? pl->d_last_vals : pl->d_val[pl->last_buf].p,
-                  pk.T, pk.tb, (uint32_t)pk.chain_begin.size() - 1, entry};
+                  pk.T, pk.tb, (uint32_t)pk.chain_begin.size() - 1, entry, nullptr};
 }
 
 // exits of every (chain, entry value): the first of the three backtrace kernels for T > 1
@@ -2180,6 +2218,348 @@ static int solve_impl(const whmec_problem *p, whmec_solution *s, int device, whm
 
 int whmec_solve(const whmec_problem *p, whmec_solution *s, int device, whmec_stats *st, char *err, size_t errlen) {
     return guarded(err, errlen, [&]() -> int { return solve_impl(p, s, device, st, err, errlen); });
+}
+
+// ---- several tables in one call ------------------------------------------------------------------------------------------
+namespace {
+
+struct BatchTable {
+    Packed pk;
+    TileSchedule ts;
+};
+
+void add_stats(whmec_stats &total, const whmec_stats &st) {
+    total.cells += st.cells;
+    total.algorithmic_bytes += st.algorithmic_bytes;
+    total.backptr_bytes += st.backptr_bytes;
+    total.state_bytes += st.state_bytes;
+    total.kernel_launches += st.kernel_launches;
+    total.n_chains += st.n_chains;
+    total.max_active = std::max(total.max_active, st.max_active);
+    total.transmissions = std::max(total.transmissions, st.transmissions);
+    total.sweep_ms += st.sweep_ms;
+    total.h2d_ms += st.h2d_ms;
+    total.d2h_ms += st.d2h_ms;
+    total.h2d_bytes += st.h2d_bytes;
+    total.d2h_bytes += st.d2h_bytes;
+    total.path_kind = (total.reserved == 0 || total.path_kind == st.path_kind) ? st.path_kind : 0;  // 0: the parts took different paths
+    total.reserved = 1;  // (marks "something was added"; cleared before the totals leave the call)
+}
+
+// One tile group: the tables `members` (all planned for the tile path) swept as one union of chains by one persistent launch,
+// backtraced by one launch, their costs reduced on the device.  *declined: the union does not fit after all (nothing was
+// solved; the caller sends the tables through the single-table path).
+int batch_tile_group(const std::vector<uint32_t> &members, std::vector<BatchTable> &tabs, whmec_solution *const *solutions, int device,
+                     int *status, std::vector<std::string> &msgs, whmec_stats *stats, whmec_stats &total, std::string &msg, bool *declined) {
+    *declined = false;
+    const uint32_t B = (uint32_t)members.size();
+    std::vector<const Packed *> pks(B);
+    std::vector<const TileSchedule *> tss(B);
+    for (uint32_t i = 0; i < B; ++i) {
+        pks[i] = &tabs[members[i]].pk;
+        tss[i] = &tabs[members[i]].ts;
+    }
+    // (declared before the plan: the plan's destructor waits for the uploads that read these arrays)
+    TileUnion un;
+    std::vector<uint32_t> pidx, costs(B);
+    merge_tile_tables(pks, tss, un);
+    std::unique_ptr<whmec_plan> pl(new whmec_plan());
+    pl->device = device;
+    pl->pk = std::move(un.pk);
+    const Packed &pk = pl->pk;
+    const uint32_t n = pk.n;
+    int rc = plan_device_setup(pl.get(), device, msg);
+    if (rc != WHMEC_OK) return rc;
+    uint64_t h2d = (uint64_t)n * sizeof(ColMeta) + ((uint64_t)B + 1) * 4;
+    CUDA_TRY(pl->d_cols.alloc(n, pl->stream));
+    CUDA_TRY(cudaMemcpyAsync(pl->d_cols.p, pk.cols.data(), (size_t)n * sizeof(ColMeta), cudaMemcpyHostToDevice, pl->stream));
+    CUDA_TRY(pl->d_path_index.alloc(n, pl->stream));
+    CUDA_TRY(pl->d_result.alloc(4, pl->stream));
+    CUDA_TRY(pl->d_table_chain.alloc((size_t)B + 1, pl->stream));
+    CUDA_TRY(pl->d_table_cost.alloc(B, pl->stream));
+    CUDA_TRY(cudaMemcpyAsync(pl->d_table_chain.p, un.table_chain.data(), ((size_t)B + 1) * 4, cudaMemcpyHostToDevice, pl->stream));
+    pl->tiles.adopt(std::move(un.ts));
+    pl->use_tiles = true;
+    rc = pl->tiles.create(pk, pl->stream, h2d, msg, pl->d_cols.p);
+    if (rc == WHMEC_ERR_UNSUPPORTED && pl->tiles.over_hbm) {
+        *declined = true;
+        msg.clear();
+        return WHMEC_OK;
+    }
+    if (rc != WHMEC_OK) return rc;
+    CUDA_TRY(cudaEventRecord(pl->evh1, pl->stream));
+    CUDA_TRY(cudaEventRecord(pl->ev0, pl->stream));
+    if ((rc = pl->tiles.sweep(pk, pl->stream, msg)) != WHMEC_OK) return rc;
+    CUDA_TRY(cudaEventRecord(pl->ev1, pl->stream));
+    if ((rc = pl->tiles.backtrace(pk, pl->stream, pl->d_path_index.p, pl->d_result.p, msg)) != WHMEC_OK) return rc;
+    if ((rc = pl->tiles.table_costs(pl->stream, pl->d_table_chain.p, B, pl->d_table_cost.p, msg)) != WHMEC_OK) return rc;
+    pidx.resize(n);
+    CUDA_TRY(cudaMemcpyAsync(pidx.data(), pl->d_path_index.p, (size_t)n * 4, cudaMemcpyDeviceToHost, pl->stream));
+    CUDA_TRY(cudaMemcpyAsync(costs.data(), pl->d_table_cost.p, (size_t)B * 4, cudaMemcpyDeviceToHost, pl->stream));
+    CUDA_TRY(cudaStreamSynchronize(pl->stream));
+    whmec_stats group{};
+    CUDA_TRY(cudaEventElapsedTime(&group.sweep_ms, pl->ev0, pl->ev1));
+    CUDA_TRY(cudaEventElapsedTime(&group.h2d_ms, pl->evh0, pl->evh1));
+    group.kernel_launches = pl->tiles.launches;
+    group.backptr_bytes = pl->tiles.backptr_bytes;
+    group.state_bytes = pl->tiles.state_bytes;
+    group.h2d_bytes = h2d;
+    group.d2h_bytes = (uint64_t)n * 4 + (uint64_t)B * 4;
+    group.path_kind = 1;
+    // the output pass of every table (a table's transmission values are all 0: one individual)
+    uint32_t longest = 0;
+    for (uint32_t i = 0; i < B; ++i) longest = std::max(longest, pks[i]->n);
+    const std::vector<uint32_t> ptv(longest, 0);
+    for (uint32_t i = 0; i < B; ++i) {  // (one table after the other: the output pass spreads every table over the host workers itself)
+        const uint32_t t = members[i];
+        solutions[t]->cost = costs[i];
+        status[t] = build_outputs(*pks[i], pidx.data() + un.table_col[i], ptv.data(), solutions[t], msgs[t]);
+    }
+    for (uint32_t i = 0; i < B; ++i) {
+        whmec_stats st = pks[i]->stats;
+        st.path_kind = 1;
+        st.backptr_bytes = tss[i]->bp_words * 4;
+        st.state_bytes = tss[i]->state_traffic_bytes;
+        group.cells += st.cells;
+        group.algorithmic_bytes += st.algorithmic_bytes;
+        group.n_chains += st.n_chains;
+        group.max_active = std::max(group.max_active, st.max_active);
+        group.transmissions = st.transmissions;
+        if (stats) stats[members[i]] = st;
+    }
+    add_stats(total, group);
+    return WHMEC_OK;
+}
+
+// One fused-trio group: the tables `members` (one trio each, every column of the fused shape) as one union of chains.  Pass 1
+// and pass 2 of the fused sweep take all chains at once (cluster size chosen from the total), the fold between them restarts at
+// every table (ped_fused_tables_prefix_kernel), the backtrace enters every table's last chain at that table's optimum.
+// *declined: the union does not fit resident or left the fused shape (nothing was solved).
+int batch_fused_group(const std::vector<uint32_t> &members, std::vector<BatchTable> &tabs, whmec_solution *const *solutions, int device,
+                      int *status, std::vector<std::string> &msgs, whmec_stats *stats, whmec_stats &total, std::string &msg, bool *declined) {
+    *declined = false;
+    const uint32_t B = (uint32_t)members.size();
+    std::vector<const Packed *> pks(B);
+    for (uint32_t i = 0; i < B; ++i) pks[i] = &tabs[members[i]].pk;
+    // (declared before the plan: the plan's destructor waits for the copies that use these arrays)
+    PackedUnion un;
+    std::vector<uint32_t> pidx, ptv, costs(B);
+    merge_column_tables(pks, un);
+    std::unique_ptr<whmec_plan> pl(new whmec_plan());
+    pl->device = device;
+    pl->pk = std::move(un.pk);
+    const Packed &pk = pl->pk;
+    const uint32_t n = pk.n, C = (uint32_t)pk.chain_begin.size() - 1;
+    int rc = plan_device_setup(pl.get(), device, msg);
+    if (rc != WHMEC_OK) return rc;
+    uint64_t h2d = ((uint64_t)B + 1 + C) * 4;
+    rc = col_create(pl.get(), false, h2d, msg);
+    if (rc == WHMEC_ERR_UNSUPPORTED || (rc == WHMEC_OK && (pl->col.path != ColPath::fused || pl->col.bounded))) {
+        *declined = true;
+        msg.clear();
+        return WHMEC_OK;
+    }
+    if (rc != WHMEC_OK) return rc;
+    CUDA_TRY(pl->d_path_index.alloc(n, pl->stream));
+    CUDA_TRY(pl->d_path_tv.alloc(n, pl->stream));
+    CUDA_TRY(pl->d_table_chain.alloc((size_t)B + 1, pl->stream));
+    CUDA_TRY(pl->d_table_end.alloc(C, pl->stream));
+    CUDA_TRY(pl->d_table_cost.alloc(B, pl->stream));
+    CUDA_TRY(cudaMemcpyAsync(pl->d_table_chain.p, un.table_chain.data(), ((size_t)B + 1) * 4, cudaMemcpyHostToDevice, pl->stream));
+    CUDA_TRY(cudaMemcpyAsync(pl->d_table_end.p, un.table_end.data(), (size_t)C * 4, cudaMemcpyHostToDevice, pl->stream));
+    CUDA_TRY(cudaEventRecord(pl->evh1, pl->stream));
+    CUDA_TRY(cudaEventRecord(pl->ev0, pl->stream));
+    if ((rc = ped_fused_pass(pl.get(), true, msg)) != WHMEC_OK) return rc;
+    ped_fused_tables_prefix_kernel<<<(B + 31) / 32, 32, 0, pl->stream>>>(pl->d_chain_rows.p, pl->d_table_chain.p, B, pl->d_chain_in.p);
+    CUDA_TRY(cudaGetLastError());
+    if ((rc = ped_fused_pass(pl.get(), false, msg)) != WHMEC_OK) return rc;
+    CUDA_TRY(cudaEventRecord(pl->ev1, pl->stream));
+    BtArgs a = bt_args(pl.get(), -1);
+    a.last_vals = pl->d_chain_out.p;
+    a.table_end = pl->d_table_end.p;
+    bt_exits_kernel<<<C * a.T, 32, 0, pl->stream>>>(a, pl->d_bt_exits.p);
+    bt_table_entries_kernel<<<(B + 31) / 32, 32, 0, pl->stream>>>(a, pl->d_bt_exits.p, pl->d_table_chain.p, B, pl->d_bt_entries.p);
+    bt_paths_kernel<<<C, 32, 0, pl->stream>>>(a, pl->d_bt_entries.p, pl->d_path_index.p, pl->d_path_tv.p, pl->d_table_cost.p);
+    CUDA_TRY(cudaGetLastError());
+    pidx.resize(n);
+    ptv.resize(n);
+    CUDA_TRY(cudaMemcpyAsync(pidx.data(), pl->d_path_index.p, (size_t)n * 4, cudaMemcpyDeviceToHost, pl->stream));
+    CUDA_TRY(cudaMemcpyAsync(ptv.data(), pl->d_path_tv.p, (size_t)n * 4, cudaMemcpyDeviceToHost, pl->stream));
+    CUDA_TRY(cudaMemcpyAsync(costs.data(), pl->d_table_cost.p, (size_t)B * 4, cudaMemcpyDeviceToHost, pl->stream));
+    CUDA_TRY(cudaStreamSynchronize(pl->stream));
+    whmec_stats group{};
+    CUDA_TRY(cudaEventElapsedTime(&group.sweep_ms, pl->ev0, pl->ev1));
+    CUDA_TRY(cudaEventElapsedTime(&group.h2d_ms, pl->evh0, pl->evh1));
+    group.kernel_launches = 3;  // pass 1, the fold, pass 2
+    group.backptr_bytes = pk.bp_words * 4;
+    group.h2d_bytes = h2d;
+    group.d2h_bytes = (uint64_t)n * 8 + (uint64_t)B * 4;
+    group.path_kind = 3;
+    for (uint32_t i = 0; i < B; ++i) {
+        const uint32_t t = members[i];
+        solutions[t]->cost = costs[i];
+        status[t] = build_outputs(*pks[i], pidx.data() + un.table_col[i], ptv.data() + un.table_col[i], solutions[t], msgs[t]);
+        whmec_stats st = pks[i]->stats;
+        st.path_kind = 3;
+        st.backptr_bytes = pks[i]->bp_words * 4;
+        group.cells += st.cells;
+        group.algorithmic_bytes += st.algorithmic_bytes;
+        group.n_chains += st.n_chains;
+        group.max_active = std::max(group.max_active, st.max_active);
+        group.transmissions = st.transmissions;
+        if (stats) stats[t] = st;
+    }
+    add_stats(total, group);
+    return WHMEC_OK;
+}
+
+int solve_batch_impl(const whmec_problem *const *problems, whmec_solution *const *solutions, uint32_t n_tables, int device, int *status,
+                     char *errs, size_t errlen, whmec_stats *stats, whmec_stats *total_out) {
+    whmec_stats total{};
+    std::vector<std::string> msgs(n_tables);
+    for (uint32_t t = 0; t < n_tables; ++t) {
+        status[t] = WHMEC_OK;
+        if (stats) stats[t] = whmec_stats{};
+    }
+    auto err_of = [&](uint32_t t) { return errs ? errs + (size_t)t * errlen : nullptr; };
+    auto fail_call = [&](int rc, const std::string &msg) {  // the call failed: every table reports why
+        for (uint32_t t = 0; t < n_tables; ++t) {
+            status[t] = rc;
+            set_err(err_of(t), errlen, msg);
+        }
+        return rc;
+    };
+    keep_host_memory();
+    std::string msg;
+    // (a failure to select the device is reported by the first table that needs it, after the host-detectable input errors,
+    // as whmec_solve does)
+    if (cudaSetDevice(device) == cudaSuccess) install_stage_hooks();
+    else cudaGetLastError();
+    // Routing.  Single-individual tables are packed and planned for the tile path here, one after the other (the packer and
+    // the planner spread every table over the host workers themselves); a table the tile planner accepts joins a tile group.  Everything else -- pedigrees, tables with an input error (the
+    // single-table path reports it with its own code and text), tables the planner declines, tables without columns -- is
+    // solved by the single-table path, one after the other.
+    const char *force = std::getenv("WHMEC_FORCE_COLUMN_KERNEL");
+    const bool forced_column = force && force[0] == '1';
+    std::vector<BatchTable> tabs(n_tables);
+    std::vector<uint8_t> tiled(n_tables, 0);
+    const char *pf_env = std::getenv("WHMEC_PED_FUSED"), *seq_env = std::getenv("WHMEC_PED_SEQUENTIAL");
+    const bool fused_on = !(pf_env && pf_env[0] == '0') && !(seq_env && seq_env[0] == '1');
+    std::vector<uint8_t> fusable(n_tables, 0);  // one trio, every column of the fused kernel's shape: joins a fused-trio group
+    for (uint32_t t = 0; t < n_tables; ++t) {
+        const whmec_problem *p = problems[t];
+        if (!p || !solutions[t]) continue;
+        std::string m;
+        BatchTable &bt = tabs[t];
+        if (p->n_trios == 1 && p->n_ind == 3 && fused_on) {
+            bool ok = pack_problem(p, bt.pk, m, true) == WHMEC_OK && bt.pk.n > 0 && bt.pk.T == PF_T && bt.pk.safe31 && bt.pk.max_d + bt.pk.tb <= 32;
+            for (uint32_t k = 0; k < bt.pk.n && ok; ++k) ok = pf_column_ok(bt.pk.cols[k], bt.pk.fn_group.data() + bt.pk.cols[k].grp_off);
+            fusable[t] = ok;
+            if (!ok) bt = BatchTable();
+            continue;
+        }
+        if (p->n_ind != 1 || p->n_trios != 0 || forced_column) continue;
+        if (pack_problem(p, bt.pk, m, false) != WHMEC_OK || bt.pk.n == 0 || bt.pk.max_d + bt.pk.tb > 32) {
+            bt = BatchTable();
+            continue;
+        }
+        plan_tiles(bt.pk, bt.ts);
+        tiled[t] = bt.ts.eligible;
+        if (!tiled[t]) bt = BatchTable();
+    }
+    // Groups: consecutive tile tables whose device memory fits together under ONE reading of the free memory (two plans
+    // created side by side would each claim all of it).  WHMEC_TILE_ARENA_BUDGET (test hook) bounds a group as it bounds a table.
+    std::vector<uint32_t> tile_ids;
+    std::vector<uint64_t> bytes, items;
+    for (uint32_t t = 0; t < n_tables; ++t)
+        if (tiled[t]) {
+            tile_ids.push_back(t);
+            bytes.push_back(tile_table_bytes(tabs[t].pk, tabs[t].ts));
+            items.push_back(tile_table_items(tabs[t].ts));
+        }
+    const uint64_t free_b = device_available_bytes(), reserve = 512ull << 20;
+    uint64_t budget = free_b > reserve ? free_b - reserve : 0;
+    if (const char *e = std::getenv("WHMEC_TILE_ARENA_BUDGET")) budget = std::min<uint64_t>(budget, std::max<uint64_t>(8, std::strtoull(e, nullptr, 10)));
+    std::vector<std::pair<uint32_t, uint32_t>> groups;
+    std::vector<uint32_t> alone;
+    cut_table_groups(bytes, items, budget, groups, alone);
+    for (uint32_t i : alone) tiled[tile_ids[i]] = 0;
+    for (const auto &g : groups) {
+        std::vector<uint32_t> members(tile_ids.begin() + g.first, tile_ids.begin() + g.second);
+        bool declined = false;  // (a group of one table runs like any other: the table is packed and planned already)
+        const int rc = batch_tile_group(members, tabs, solutions, device, status, msgs, stats, total, msg, &declined);
+        if (rc != WHMEC_OK) return fail_call(rc, msg);
+        for (uint32_t t : members) {
+            if (declined) tiled[t] = 0;
+            else set_err(err_of(t), errlen, msgs[t]);
+            tabs[t] = BatchTable();
+        }
+    }
+    // Fused-trio groups, cut the same way: WHMEC_COLUMN_ARENA_BUDGET (test hook) bounds a group as it bounds a table's arena.
+    {
+        std::vector<uint32_t> ids;
+        std::vector<uint64_t> fbytes, fitems;
+        for (uint32_t t = 0; t < n_tables; ++t)
+            if (fusable[t]) {
+                ids.push_back(t);
+                fbytes.push_back(column_table_bytes(tabs[t].pk));
+                fitems.push_back(column_table_functions(tabs[t].pk));
+            }
+        uint64_t fbudget = free_b > reserve ? free_b - reserve : 0;
+        if (const char *e = std::getenv("WHMEC_COLUMN_ARENA_BUDGET")) fbudget = std::min<uint64_t>(fbudget, std::max<uint64_t>(8, std::strtoull(e, nullptr, 10)));
+        cut_table_groups(fbytes, fitems, fbudget, groups, alone);
+        for (uint32_t i : alone) fusable[ids[i]] = 0;
+        for (const auto &g : groups) {
+            std::vector<uint32_t> members(ids.begin() + g.first, ids.begin() + g.second);
+            bool declined = false;
+            const int rc = batch_fused_group(members, tabs, solutions, device, status, msgs, stats, total, msg, &declined);
+            if (rc != WHMEC_OK) return fail_call(rc, msg);
+            for (uint32_t t : members) {
+                if (declined) fusable[t] = 0;
+                else set_err(err_of(t), errlen, msgs[t]);
+                tabs[t] = BatchTable();
+            }
+        }
+    }
+    for (uint32_t t = 0; t < n_tables; ++t) {
+        if (tiled[t] || fusable[t]) continue;
+        tabs[t] = BatchTable();
+        if (!problems[t] || !solutions[t]) {
+            status[t] = WHMEC_ERR_INPUT;
+            set_err(err_of(t), errlen, "null problem or solution");
+            continue;
+        }
+        whmec_stats st{};
+        char local[512] = {0};
+        const int rc = guarded(local, sizeof local, [&]() -> int { return solve_impl(problems[t], solutions[t], device, &st, local, sizeof local); });
+        if (rc == WHMEC_ERR_CUDA) return fail_call(rc, local);
+        status[t] = rc;
+        set_err(err_of(t), errlen, local);
+        if (rc != WHMEC_OK) continue;
+        add_stats(total, st);
+        st.sweep_ms = st.h2d_ms = st.d2h_ms = 0;
+        if (stats) stats[t] = st;
+    }
+    total.reserved = 0;
+    if (total_out) *total_out = total;
+    return WHMEC_OK;
+}
+
+}  // namespace
+
+int whmec_solve_batch(const whmec_problem *const *problems, whmec_solution *const *solutions, uint32_t n_tables, int device, int *status,
+                      char *errs, size_t errlen, whmec_stats *stats, whmec_stats *total) {
+    if (total) *total = whmec_stats{};
+    if (n_tables == 0) return WHMEC_OK;
+    if (!problems || !solutions || !status) return WHMEC_ERR_INPUT;
+    char local[512] = {0};
+    const int rc = guarded(local, sizeof local, [&]() -> int { return solve_batch_impl(problems, solutions, n_tables, device, status, errs, errlen, stats, total); });
+    if (local[0])  // an exception left the driver (out of host memory): the call failed, every table reports why
+        for (uint32_t t = 0; t < n_tables; ++t) {
+            status[t] = rc;
+            set_err(errs ? errs + (size_t)t * errlen : nullptr, errlen, local);
+        }
+    return rc;
 }
 
 }  // extern "C"

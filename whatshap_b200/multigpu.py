@@ -825,3 +825,50 @@ def genotype_table(prob: FlatProblem, device: int = 0, devices: Optional[Sequenc
 
     chosen = table_devices(device, devices)
     return _lib.genotype(prob, device=device) if chosen is None else genotype_on_devices(prob, chosen)
+
+
+def solve_tables(problems: Sequence[FlatProblem], device: int = 0, devices: Optional[Sequence[int]] = None, with_stats: bool = False):
+    """Several tables at once: per table, in input order, its `FlatSolution` or the exception `solve_table` would have raised
+    for it (an input error, a Mendelian conflict, a refusal; a failure of the device raises, whatever the length of the list).
+    On one device this is `_lib.solve_batch` (tables share the GPU's sweeps).  With `devices` / WHMEC_DEVICES whole tables go
+    to devices by longest-processing-time-first on their DP cells sum 2^a * T (`block_work`, `assign_blocks`), one
+    `whmec_solve_batch` per device on that device's host thread.  A single table behaves like `solve_table`, including being
+    spread over the devices.  `with_stats`: (results, per-table stats) instead."""
+    from . import _lib
+
+    problems = list(problems)
+    chosen = table_devices(device, devices)
+    distinct = sorted(set(chosen)) if chosen is not None else [device]
+    out: list = [None] * len(problems)
+    stats: list = [{} for _ in problems]
+    if len(problems) == 1 and len(distinct) > 1:
+        try:
+            out[0], stats[0] = solve_table(problems[0], device, devices)
+        except RuntimeError as e:  # MendelianConflict, input errors, Unsupported: the table's result
+            if str(e).startswith("CUDA failure"):
+                raise
+            out[0] = e
+    elif len(distinct) == 1 or not problems:
+        out, (stats, _) = _lib.solve_batch(problems, device=distinct[0], with_stats=True)
+    else:
+        work = np.array([float(block_work(p, [(0, p.n_cols)])[0]) * 4.0 ** p.n_trios for p in problems])
+        shares = assign_blocks(work, len(distinct))
+        jobs = [(lambda ids=ids, d=d: _lib.solve_batch([problems[i] for i in ids], device=d, with_stats=True)) if ids else None
+                for ids, d in zip(shares, distinct)]
+        results, errors = _run_on_devices(distinct, jobs)
+        for e in errors:
+            if e is not None:
+                raise e
+        for ids, res in zip(shares, results):
+            if res is not None:
+                for i, r, st in zip(ids, res[0], res[1][0]):
+                    out[i], stats[i] = r, st
+    return (out, stats) if with_stats else out
+
+
+def finish_batch(results: list, return_exceptions: bool) -> None:
+    """The error contract of the `batch` classmethods: without `return_exceptions`, the error of the lowest-index failing table."""
+    if not return_exceptions:
+        for r in results:
+            if isinstance(r, BaseException):
+                raise r
