@@ -29,8 +29,6 @@ constexpr int NT = 1024;  // threads per tile
 constexpr uint32_t TILE_ENTRIES = 1u << TILE_SMAX;
 
 constexpr uint32_t TC_CHUNK = 16;  // column descriptors staged in shared memory at a time
-constexpr uint32_t BULK_MAX_GA = 6;     // bulk-copy hand-off: at most 2^6 chunks ...
-constexpr uint32_t BULK_MIN_J = 5;      // ... of at least 2^5 entries (128 bytes)
 constexpr uint32_t BULK_SKEW = 4;       // words of skew between consecutive chunks in the staging buffer (keeps 16-byte alignment)
 constexpr uint32_t STAGE_PAD_WORDS = BULK_SKEW << BULK_MAX_GA;
 
@@ -304,9 +302,6 @@ __device__ __forceinline__ void steady_columns(TileSmem &S, uint32_t ncol, uint3
         col_phase ^= 1u;
     }
 }
-
-// Tile-major hand-offs whose chunks are at least 128 bytes travel as one bulk copy per producer tile.
-__device__ __forceinline__ bool bulk_handoff(uint32_t gA, uint32_t jb) { return gA <= BULK_MAX_GA && jb >= BULK_MIN_J; }
 
 // Bulk version of stage_tile_async (called by warp 0 only): chunk tA lands at stage + tA * (2^j + BULK_SKEW), in the
 // producer's order -- ascending for a computed producer tile, for an uncomputed one (mirrored producer) the chunk of the

@@ -17,6 +17,12 @@ constexpr uint32_t TILE_TL_BITS = TILE_MMAX < 7 ? 2 : 7;
 constexpr uint32_t TILE_TL_SIZE = 1u << TILE_TL_BITS;              // 128
 constexpr uint32_t TILE_TH_SIZE = 1u << (TILE_MMAX - TILE_TL_BITS);  // 256
 
+// Tile-major hand-offs (Panel::in_layout == 1) whose chunks are at least 128 bytes travel as one bulk copy per producer tile;
+// smaller chunks are gathered element by element (tile.cu).  The planner's tests count the panels of either kind with this rule.
+constexpr uint32_t BULK_MAX_GA = 6;     // bulk-copy hand-off: at most 2^6 chunks ...
+constexpr uint32_t BULK_MIN_J = 5;      // ... of at least 2^5 entries (128 bytes)
+WHMEC_HD bool bulk_handoff(uint32_t gA, uint32_t jb) { return gA <= BULK_MAX_GA && jb >= BULK_MIN_J; }
+
 struct TileCtx {
     const TileCol *tc;
     uint32_t tile;

@@ -357,12 +357,13 @@ def random_problem(
 
 
 def het_path_cost(prob: FlatProblem, path_index: np.ndarray) -> int:
-    """MEC cost of a given bipartition path for an all-heterozygous single individual:
+    """MEC cost of a given bipartition path for a single individual with trusted genotypes:
     sum over columns of min(D, W - D), D = weight of the reads whose allele disagrees with the
-    side they are on (closed form of pedigreecolumncostcomputer.cpp:101-114 for genotype 0/1).
+    side they are on (closed form of pedigreecolumncostcomputer.cpp:101-114 for genotype 0/1);
+    at a homozygous site (0/0 or 1/1) both sides carry its allele, so D alone.
     Used as a size-independent consistency check of large GPU runs: the reported optimal cost
     must be the cost of the reported path."""
-    assert prob.n_ind == 1 and not prob.distrust and np.all(prob.gt == 1)
+    assert prob.n_ind == 1 and not prob.distrust and np.all(prob.gt <= 2)
     n = prob.n_cols
     lens = np.diff(prob.read_off.astype(np.int64))
     rid = np.repeat(np.arange(prob.n_reads), lens)
@@ -389,10 +390,12 @@ def het_path_cost(prob: FlatProblem, path_index: np.ndarray) -> int:
     w = prob.ent_phred.astype(np.int64)
     al = prob.ent_allele.astype(np.int64)
     valid = al < 2
-    mismatch = (al != side) & valid  # het assignment (side 0 -> allele 0, side 1 -> allele 1)
+    gt = prob.gt[0].astype(np.int64)
+    # het assignment (side 0 -> allele 0, side 1 -> allele 1); homozygous: allele gt / 2 on both sides
+    mismatch = np.where(gt[cols] == 1, al != side, al != gt[cols] // 2) & valid
     D = np.bincount(cols, weights=np.where(mismatch, w, 0), minlength=n)
     W = np.bincount(cols, weights=np.where(valid, w, 0), minlength=n)
-    return int(np.minimum(D, W - D).sum())
+    return int(np.where(gt == 1, np.minimum(D, W - D), D).sum())
 
 
 def genotyping_problem(
