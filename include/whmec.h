@@ -175,6 +175,24 @@ int whmec_solve_batch(const whmec_problem *const *problems, whmec_solution *cons
  * passes, st->kernel_launches includes the repeated backward sweeps. */
 int whmec_genotype(const whmec_problem *p, double *likelihoods, int device, whmec_stats *st_or_null, char *err, size_t errlen);
 
+/* Many genotyping tables in one call (`whatshap genotype` builds one GenotypeDPTable per chromosome x family; with a
+ * multi-sample VCF and no pedigree, every sample is a family of its own).  likelihoods[t] receives what whmec_genotype writes
+ * for problems[t] ([n_ind][n_cols][3] doubles).  Tables are cut, in list order, into groups whose backward tables, projection
+ * buffers and inputs fit the budget whmec_genotype uses (the free HBM, or WHMEC_GENOTYPE_ARENA_BUDGET); one group is one
+ * upload and one step list: launch s advances the s-th column of every chain of a single individual and of every pedigree
+ * table of the group, whatever its T, so a group costs 2 x (backward + forward steps of its longest chain or pedigree table)
+ * launches.  A table that does not fit a group alone runs inside the call through whmec_genotype's own path (memory-bounded
+ * mode included).  Errors are per table: status[t] and the message at errs + t * errlen (errs may be NULL) are what
+ * whmec_genotype returns for table t.  The return value is WHMEC_ERR_INPUT for null arguments, WHMEC_ERR_CUDA for a device
+ * failure (then every status holds it and every message the reason; running out of host memory while grouping or uploading
+ * fails the call the same way, with WHMEC_ERR_UNSUPPORTED, as in whmec_solve_batch), WHMEC_OK otherwise; n_tables == 0 does
+ * nothing.  stats (optional, [n_tables]): cells,
+ * T, path_kind 4 and back-pointer bytes (backward tables) of every table, times 0; total (optional): sweep time and kernel
+ * launches of the whole call. */
+int whmec_genotype_batch(const whmec_problem *const *problems, double *const *likelihoods /* [n_tables] -> [n_ind][n_cols][3] */,
+                         uint32_t n_tables, int device, int *status /* [n_tables] */, char *errs /* [n_tables][errlen] or NULL */,
+                         size_t errlen, whmec_stats *stats_or_null /* [n_tables] */, whmec_stats *total_or_null);
+
 /* Per-column genotype priors of one sample's reads, the step `whatshap genotype` runs before the DP above
  * (compute_genotypes, src/genotyper.cpp:12-54, bound at whatshap/core.pyx:602-617): every read entry multiplies a
  * (hom-ref, het, hom-alt) distribution by the likelihood of its allele with error max(0.05, 10^(-phred/10)), renormalising

@@ -43,6 +43,7 @@ EXPORTS = (
     "whmec_selector_bridge",
     "whmec_read_sort_key",
     "whmec_genotype",
+    "whmec_genotype_batch",
     "whmec_genotype_segment_create",
     "whmec_genotype_segment_transfer",
     "whmec_genotype_segment_run",
@@ -83,6 +84,9 @@ def lib() -> C.CDLL:
     L.whmec_solve_batch.restype = C.c_int
     L.whmec_genotype.argtypes = [C.POINTER(CProblem), C.POINTER(C.c_double), C.c_int, C.POINTER(CStats), C.c_char_p, C.c_size_t]
     L.whmec_genotype.restype = C.c_int
+    L.whmec_genotype_batch.argtypes = [C.POINTER(C.POINTER(CProblem)), C.POINTER(C.POINTER(C.c_double)), C.c_uint32, C.c_int, C.POINTER(C.c_int),
+                                       C.c_char_p, C.c_size_t, C.POINTER(CStats), C.POINTER(CStats)]
+    L.whmec_genotype_batch.restype = C.c_int
     L.whmec_compute_genotypes.argtypes = [C.POINTER(CProblem), C.POINTER(C.c_double), C.POINTER(C.c_int8), C.c_char_p, C.c_size_t]
     L.whmec_compute_genotypes.restype = C.c_int
     L.whmec_heuristic.argtypes = [C.POINTER(CProblem), C.c_uint32, C.c_int, C.POINTER(CHeuristicSolution), C.c_char_p, C.c_size_t]
@@ -177,6 +181,36 @@ def genotype(prob: FlatProblem, device: int = 0) -> Tuple[np.ndarray, dict]:
     rc = lib().whmec_genotype(C.byref(cp), out.ctypes.data_as(C.POINTER(C.c_double)), device, C.byref(st), err, len(err))
     raise_for(rc, err.value.decode())
     return out, st.as_dict()
+
+
+def genotype_batch(problems: Sequence[FlatProblem], device: int = 0, with_stats: bool = False):
+    """Several tables through one `whmec_genotype_batch`: a list with, per table and in input order, its likelihoods
+    [n_ind, n_cols, 3] -- what `genotype` gives for it alone -- or the exception `genotype` would have raised for it (the other
+    tables are still genotyped).  A failure of the call itself (no device, a CUDA error) raises.  `with_stats`: also returns
+    (per-table stats, totals of the call)."""
+    n = len(problems)
+    outs = [np.zeros((p.n_ind, p.n_cols, 3), np.float64) for p in problems]
+    cps = [p.as_c() for p in problems]
+    pp = (C.POINTER(CProblem) * max(n, 1))(*[C.pointer(c) for c in cps])
+    lp = (C.POINTER(C.c_double) * max(n, 1))(*[o.ctypes.data_as(C.POINTER(C.c_double)) for o in outs])
+    status = (C.c_int * max(n, 1))()
+    errlen = 512
+    errs = C.create_string_buffer(errlen * max(n, 1))
+    stats, total = (CStats * max(n, 1))(), CStats()
+    rc = lib().whmec_genotype_batch(pp, lp, n, device, status, errs, errlen, stats, C.byref(total))
+    messages = [errs.raw[t * errlen:(t + 1) * errlen].split(b"\0", 1)[0].decode() for t in range(n)]
+    if rc != 0:
+        raise_for(rc, messages[0] if messages else "whmec_genotype_batch: invalid arguments")
+    out: List[Union[np.ndarray, Exception]] = []
+    for t in range(n):
+        try:
+            raise_for(int(status[t]), messages[t])
+            out.append(outs[t])
+        except Exception as e:  # noqa: BLE001 - handed to the caller in the table's place
+            out.append(e)
+    if with_stats:
+        return out, ([stats[t].as_dict() for t in range(n)], total.as_dict())
+    return out
 
 
 def heuristic(prob: FlatProblem, row_limit: int = 256, allow_mutations: bool = True) -> HeuristicSolution:

@@ -204,6 +204,20 @@ def flatten_objects(readset, recombcost, pedigree, distrust_genotypes: bool = Fa
     ), ids
 
 
+def _run_tables(problems, solver, tables_fn, device, devices):
+    """Results of the `batch` classmethods of the swap-in classes (no per-table stats): `solver` on every problem, an exception
+    in the table's place, or `tables_fn` (`multigpu.solve_tables` / `genotype_tables`) over all of them."""
+    if not solver:
+        return tables_fn(problems, device, devices), None
+    results = []
+    for p in problems:
+        try:
+            results.append(solver(p))
+        except Exception as e:  # noqa: BLE001
+            results.append(e)
+    return results, None
+
+
 def make_dp_table_class(core_module, solver=None):
     """A `PedigreeDPTable` look-alike (same constructor, same three methods, `whatshap/types.py:7-15`)
     that solves on the GPU and answers with `core_module`'s own Read / ReadSet objects.
@@ -221,34 +235,12 @@ def make_dp_table_class(core_module, solver=None):
         @classmethod
         def batch(cls, tables, device=0, devices=None, return_exceptions=False):
             """Several tables in one call (`core.PedigreeDPTable.batch`): `tables` holds constructor argument tuples."""
-            objs = []
-            for args in tables:
-                try:
-                    obj = cls.__new__(cls)
-                    obj.pedigree = args[2]
-                    obj._problem, obj._ids = flatten_objects(args[0], args[1], args[2], args[3] if len(args) > 3 else False,
-                                                             args[4] if len(args) > 4 else None)
-                    objs.append(obj)
-                except Exception as e:  # noqa: BLE001 - reported in the table's place, after the others ran
-                    objs.append(e)
-            good = [i for i, o in enumerate(objs) if not isinstance(o, BaseException)]
-            problems = [objs[i]._problem for i in good]
-            if solver:
-                solutions = []
-                for p in problems:
-                    try:
-                        solutions.append(solver(p))
-                    except Exception as e:  # noqa: BLE001
-                        solutions.append(e)
-            else:
-                solutions = multigpu.solve_tables(problems, device, devices)
-            for i, sol in zip(good, solutions):
-                if isinstance(sol, BaseException):
-                    objs[i] = sol
-                else:
-                    objs[i]._solution = sol
-            multigpu.finish_batch(objs, return_exceptions)
-            return objs
+            def build(obj, args):
+                obj.pedigree = args[2]
+                obj._problem, obj._ids = flatten_objects(args[0], args[1], args[2], args[3] if len(args) > 3 else False, args[4] if len(args) > 4 else None)
+
+            return multigpu.batch_objects(cls, tables, build, lambda problems: _run_tables(problems, solver, multigpu.solve_tables, device, devices),
+                                          "_solution", return_exceptions)
 
         def get_super_reads(self):
             prob, sol = self._problem, self._solution
@@ -339,6 +331,17 @@ def make_genotype_table_class(core_module, solver=None):
             self._problem, self._ids = flatten_objects(readset, recombcost, pedigree, True, positions)
             run = solver or (lambda p: multigpu.genotype_table(p)[0])
             self._likelihoods = run(self._problem)
+
+        @classmethod
+        def batch(cls, tables, device=0, devices=None, return_exceptions=False):
+            """Several tables in one call (`core.GenotypeDPTable.batch`): `tables` holds constructor argument tuples."""
+            def build(obj, args):
+                obj.pedigree = args[3]
+                obj.numeric_sample_ids = args[0]
+                obj._problem, obj._ids = flatten_objects(args[1], args[2], args[3], True, args[4] if len(args) > 4 else None)
+
+            return multigpu.batch_objects(cls, tables, build, lambda problems: _run_tables(problems, solver, multigpu.genotype_tables, device, devices),
+                                          "_likelihoods", return_exceptions)
 
         def get_genotype_likelihoods(self, sample_id, pos):
             index = self._ids.index(self.numeric_sample_ids[sample_id])

@@ -762,30 +762,18 @@ class PedigreeDPTable:
         behaves exactly like `cls(*arguments)`.  A table that fails does not stop the others: afterwards the error of the
         lowest-index failing table is raised, with the type and text the constructor would have raised; with
         `return_exceptions` the exception instance takes the table's place instead."""
-        objs: list = []
-        for args in tables:
-            try:
-                readset, recombcost, pedigree = args[0], args[1], args[2]
-                if not isinstance(readset, ReadSet):
-                    raise TypeError("Argument 'readset' has incorrect type")
-                if not isinstance(pedigree, Pedigree):
-                    raise TypeError("Argument 'pedigree' has incorrect type")
-                obj = cls.__new__(cls)
-                obj.pedigree = pedigree
-                obj._problem = _flatten(readset, recombcost, pedigree, bool(args[3]) if len(args) > 3 else False, args[4] if len(args) > 4 else None)
-                obj.stats = {}
-                objs.append(obj)
-            except Exception as e:  # noqa: BLE001 - reported in the table's place, after the others ran
-                objs.append(e)
-        good = [i for i, o in enumerate(objs) if not isinstance(o, BaseException)]
-        solutions, stats = multigpu.solve_tables([objs[i]._problem for i in good], device, devices, with_stats=True)
-        for i, sol, st in zip(good, solutions, stats):
-            if isinstance(sol, BaseException):
-                objs[i] = sol
-            else:
-                objs[i]._solution, objs[i].stats = sol, st  # (times are 0: the tables shared their sweeps)
-        multigpu.finish_batch(objs, return_exceptions)
-        return objs
+        def build(obj, args):
+            readset, recombcost, pedigree = args[0], args[1], args[2]
+            if not isinstance(readset, ReadSet):
+                raise TypeError("Argument 'readset' has incorrect type")
+            if not isinstance(pedigree, Pedigree):
+                raise TypeError("Argument 'pedigree' has incorrect type")
+            obj.pedigree = pedigree
+            obj._problem = _flatten(readset, recombcost, pedigree, bool(args[3]) if len(args) > 3 else False, args[4] if len(args) > 4 else None)
+            obj.stats = {}
+
+        return multigpu.batch_objects(cls, tables, build, lambda problems: multigpu.solve_tables(problems, device, devices, with_stats=True),
+                                      "_solution", return_exceptions)
 
     def get_super_reads(self) -> Tuple[List[ReadSet], List[int]]:
         """One ReadSet per individual (pedigree order) holding `superread_0_<k>` and
@@ -907,6 +895,27 @@ class GenotypeDPTable:
         # the priors travel in the `gl` array of the flat problem (as they do for distrusted genotypes)
         self._problem = _flatten(readset, recombcost, pedigree, True, positions)
         self._likelihoods, self.stats = multigpu.genotype_table(self._problem, device, devices)
+
+    @classmethod
+    def batch(cls, tables, device: int = 0, devices=None, return_exceptions: bool = False) -> list:
+        """Several tables in one call, sharing the GPU's launches (`multigpu.genotype_tables`, `whmec_genotype_batch`).  `tables`
+        is a sequence of constructor argument tuples `(numeric_sample_ids, readset, recombcost, pedigree[, positions])`; every
+        returned object answers `get_genotype_likelihoods` exactly like `cls(*arguments)`.  A table that fails does not stop the
+        others: afterwards the error of the lowest-index failing table is raised, with the type and text the constructor would
+        have raised; with `return_exceptions` the exception instance takes the table's place instead."""
+        def build(obj, args):
+            numeric_sample_ids, readset, recombcost, pedigree = args[0], args[1], args[2], args[3]
+            if not isinstance(readset, ReadSet):
+                raise TypeError("Argument 'readset' has incorrect type")
+            if not isinstance(pedigree, Pedigree):
+                raise TypeError("Argument 'pedigree' has incorrect type")
+            obj.pedigree = pedigree
+            obj.numeric_sample_ids = numeric_sample_ids
+            obj._problem = _flatten(readset, recombcost, pedigree, True, args[4] if len(args) > 4 else None)
+            obj.stats = {}
+
+        return multigpu.batch_objects(cls, tables, build, lambda problems: multigpu.genotype_tables(problems, device, devices, with_stats=True),
+                                      "_likelihoods", return_exceptions)
 
     def get_genotype_likelihoods(self, sample_id, pos: int) -> PhredGenotypeLikelihoods:
         """Likelihoods of 0/0, 0/1, 1/1 of `sample_id` at column `pos` (src/genotypedptable.cpp:445-451)."""

@@ -14,6 +14,9 @@
 // A pedigree table can also be split into segments of whole chains, one per GPU (whmec_genotype_segment_*, DESIGN §4.5): a
 // forward-only transfer pass per segment (gl_transfer_kernel) gives the T x T matrix that carries the T values across the
 // cut, the caller folds the matrices, and each segment runs the passes above from its true inputs.
+// Many tables in one call (whmec_genotype_batch, DESIGN §4.9): the sub-tables of every table of a group (a single individual's
+// chains, a pedigree's whole table) share one step list, swept by gl_batch_backward_kernel / gl_batch_forward_kernel, which read
+// each step's table from a descriptor (gl_batch.h), and the same gl_scale_kernel.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -24,6 +27,7 @@
 #include <string>
 #include <vector>
 
+#include "gl_batch.h"
 #include "gl_pack.h"
 #include "tile.cuh"  // device_available_bytes
 
@@ -102,6 +106,46 @@ __global__ void __launch_bounds__(1024) gl_scale_kernel(const GlStep *steps, dou
     }
     double *c = pool + st.prev_off;
     for (uint64_t i = threadIdx.x; i < st.n_clear; i += blockDim.x) c[i] = 0.0;
+}
+
+// A group of whmec_genotype_batch (gl_batch_plan): grid.y = the steps of this launch, each of its own table (tables[step_table[y]]:
+// singles, trios and larger pedigrees share a launch; a CTA never mixes tables); grid.x covers the widest column among them.
+// The cells are those of gl_backward_kernel / gl_forward_kernel on the table's view of the group's concatenated inputs.
+__global__ void __launch_bounds__(GL_THREADS) gl_batch_backward_kernel(GlBatchInputs in, const GlBatchTable *tables, const GlStep *steps,
+                                                                       const uint32_t *step_table, double *beta) {
+    const GlStep st = steps[blockIdx.y];
+    const uint64_t x = (uint64_t)blockIdx.x * GL_THREADS + threadIdx.x;
+    if (x >= ((uint64_t)1 << st.cells_log2)) return;
+    const GlBatchTable d = tables[step_table[blockIdx.y]];
+    const GlView v = gl_batch_view(in, d);
+    gl_backward_cell(v, st.k, (uint32_t)x, beta + d.beta_base + v.cols[st.k].beta_off, beta + st.cur_off, AtomicAdd());
+}
+
+// acc: every table's posterior accumulators, [n_cols][n_ind * 3] from its acc_base
+__global__ void __launch_bounds__(GL_THREADS) gl_batch_forward_kernel(GlBatchInputs in, const GlBatchTable *tables, const GlStep *steps,
+                                                                      const uint32_t *step_table, double *F, const double *beta, double *acc) {
+    __shared__ double s_acc[GL_MAX_IND * 3];
+    const GlStep st = steps[blockIdx.y];
+    if ((uint64_t)blockIdx.x * GL_THREADS >= ((uint64_t)1 << st.cells_log2)) return;  // whole block beyond this column (uniform)
+    const GlBatchTable d = tables[step_table[blockIdx.y]];
+    const GlView v = gl_batch_view(in, d);
+    const uint32_t n_acc = v.n_ind * 3;
+    const double *beta_k = beta + d.beta_base + v.cols[st.k].beta_off;
+    double *acc_k = acc + d.acc_base + (size_t)st.k * n_acc;
+    if (threadIdx.x < n_acc) s_acc[threadIdx.x] = 0.0;
+    __syncthreads();
+    double lacc[GL_MAX_IND * 3];
+    for (uint32_t e = 0; e < n_acc; ++e) lacc[e] = 0.0;
+    const uint64_t x = (uint64_t)blockIdx.x * GL_THREADS + threadIdx.x;
+    if (x < ((uint64_t)1 << st.cells_log2))
+        gl_forward_cell(v, st.k, (uint32_t)x, F + st.prev_off, F + st.cur_off, beta_k, lacc, AtomicAdd());
+    for (uint32_t e = 0; e < n_acc; ++e) {
+        double s = lacc[e];
+        for (int off = 16; off > 0; off >>= 1) s += __shfl_down_sync(0xFFFFFFFFu, s, off);
+        if ((threadIdx.x & 31) == 0 && s != 0.0) atomicAdd(&s_acc[e], s);
+    }
+    __syncthreads();
+    if (threadIdx.x < n_acc && s_acc[threadIdx.x] != 0.0) atomicAdd(&acc_k[threadIdx.x], s_acc[threadIdx.x]);
 }
 
 // Transfer pass of a segment (gl_transfer_plan): one column for the n_in input rows of a batch.  grid.x covers the column.
@@ -388,6 +432,192 @@ int guarded(F &&fn, char *err, size_t errlen) {
     return rc;
 }
 
+void set_err(char *err, size_t errlen, const std::string &msg) {
+    if (err && errlen) {
+        std::strncpy(err, msg.c_str(), errlen - 1);
+        err[errlen - 1] = 0;
+    }
+}
+
+void add_stats(whmec_stats &total, const whmec_stats &st) {
+    total.cells += st.cells;
+    total.algorithmic_bytes += st.algorithmic_bytes;
+    total.backptr_bytes += st.backptr_bytes;
+    total.kernel_launches += st.kernel_launches;
+    total.n_chains += st.n_chains;
+    total.max_active = std::max(total.max_active, st.max_active);
+    total.transmissions = std::max(total.transmissions, st.transmissions);
+    total.sweep_ms += st.sweep_ms;
+    total.h2d_bytes += st.h2d_bytes;
+    total.d2h_bytes += st.d2h_bytes;
+    total.path_kind = 4;
+}
+
+// One group of whmec_genotype_batch on stream s: one upload (concatenated inputs, descriptors, step list), one clear of the work
+// buffer (backward store, F pool, accumulators), the launches of the group's step list, one copy of every member's posteriors
+// back, each normalised into its caller's array.
+int run_batch_group(cudaStream_t s, const GlBatchGroup &gp, const std::vector<Packed> &pks, const std::vector<GlPacked> &gs, double *const *likelihoods,
+                    whmec_stats *stats, whmec_stats &total, std::string &msg) {
+    std::vector<uint8_t> blob;
+    auto put = [&](const void *src, size_t bytes) {  // 16-byte aligned sections
+        const size_t at = (blob.size() + 15) & ~(size_t)15;
+        blob.resize(at + bytes);
+        if (bytes) std::memcpy(blob.data() + at, src, bytes);
+        return at;
+    };
+    const size_t o_cols = put(gp.cols.data(), gp.cols.size() * sizeof(GlCol)), o_eps = put(gp.eps.data(), gp.eps.size() * 8),
+                 o_trans = put(gp.trans.data(), gp.trans.size() * 8), o_q = put(gp.q.data(), gp.q.size() * 8),
+                 o_allele = put(gp.allele.data(), gp.allele.size()), o_ind = put(gp.ind.data(), gp.ind.size()), o_h2p = put(gp.h2p.data(), gp.h2p.size()),
+                 o_tables = put(gp.tables.data(), gp.tables.size() * sizeof(GlBatchTable)),
+                 o_steps = put(gp.steps.data(), gp.steps.size() * sizeof(GlStep)),
+                 o_step_table = put(gp.step_table.data(), gp.step_table.size() * 4);
+    const uint64_t work = gp.store_doubles + gp.f_pool_doubles + gp.acc_doubles;
+    Buffers W;
+    W.stream = s;
+    W.owns_stream = false;
+    uint8_t *d_blob = nullptr;
+    double *d_work = nullptr;
+    CUDA_TRY(W.alloc(&d_blob, blob.size()));
+    CUDA_TRY(W.alloc(&d_work, work));
+    CUDA_TRY(cudaMemcpyAsync(d_blob, blob.data(), blob.size(), cudaMemcpyHostToDevice, s));
+    CUDA_TRY(cudaMemsetAsync(d_work, 0, work * 8, s));
+    const GlBatchInputs in{(const GlCol *)(d_blob + o_cols),  (const double *)(d_blob + o_eps), d_blob + o_allele,          d_blob + o_ind,
+                           (const int8_t *)(d_blob + o_h2p), (const double *)(d_blob + o_trans), (const double *)(d_blob + o_q)};
+    const GlBatchTable *d_tables = (const GlBatchTable *)(d_blob + o_tables);
+    const GlStep *d_steps = (const GlStep *)(d_blob + o_steps);
+    const uint32_t *d_step_table = (const uint32_t *)(d_blob + o_step_table);
+    double *d_beta = d_work, *d_F = d_work + gp.store_doubles, *d_acc = d_F + gp.f_pool_doubles;
+    auto widest = [&](uint32_t e0, uint32_t e1) {
+        uint32_t a_max = 0;
+        for (uint32_t e = e0; e < e1; ++e) a_max = std::max(a_max, gp.steps[e].cells_log2);
+        return (unsigned)((((uint64_t)1 << a_max) + GL_THREADS - 1) / GL_THREADS);
+    };
+    Timer tm;
+    CUDA_TRY(tm.start(s));
+    uint32_t launches = 0;
+    for (size_t l = 0; l + 1 < gp.bwd_begin.size(); ++l)
+        for (uint32_t e0 = gp.bwd_begin[l]; e0 < gp.bwd_begin[l + 1]; e0 += GL_MAX_GRID_Y) {
+            const uint32_t e1 = std::min(gp.bwd_begin[l + 1], e0 + GL_MAX_GRID_Y);
+            gl_batch_backward_kernel<<<dim3(widest(e0, e1), e1 - e0), GL_THREADS, 0, s>>>(in, d_tables, d_steps + e0, d_step_table + e0, d_beta);
+            gl_scale_kernel<<<e1 - e0, 1024, 0, s>>>(d_steps + e0, d_beta);
+            launches += 2;
+        }
+    for (size_t l = 0; l + 1 < gp.fwd_begin.size(); ++l)
+        for (uint32_t e0 = gp.fwd_begin[l]; e0 < gp.fwd_begin[l + 1]; e0 += GL_MAX_GRID_Y) {
+            const uint32_t e1 = std::min(gp.fwd_begin[l + 1], e0 + GL_MAX_GRID_Y);
+            gl_batch_forward_kernel<<<dim3(widest(e0, e1), e1 - e0), GL_THREADS, 0, s>>>(in, d_tables, d_steps + e0, d_step_table + e0, d_F, d_beta,
+                                                                                         d_acc);
+            gl_scale_kernel<<<e1 - e0, 1024, 0, s>>>(d_steps + e0, d_F);
+            launches += 2;
+        }
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaEventRecord(tm.ev1, s));
+    std::vector<double> acc(gp.acc_doubles);
+    CUDA_TRY(cudaMemcpyAsync(acc.data(), d_acc, acc.size() * 8, cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaStreamSynchronize(s));
+    whmec_stats group{};
+    CUDA_TRY(cudaEventElapsedTime(&group.sweep_ms, tm.ev0, tm.ev1));
+    group.kernel_launches = launches;
+    group.h2d_bytes = blob.size();
+    group.d2h_bytes = acc.size() * 8;
+    add_stats(total, group);
+    for (size_t m = 0; m < gp.members.size(); ++m) {
+        const uint32_t t = gp.members[m];
+        const GlBatchTable &d = gp.tables[m];
+        gl_normalise(acc.data() + d.acc_base, d.n_cols, d.n_ind, likelihoods[t]);
+        whmec_stats st = pks[t].stats;  // times and launches: the group's, in `total`
+        st.path_kind = 4;
+        st.backptr_bytes = gs[t].beta_doubles * 8;
+        add_stats(total, st);
+        if (stats) stats[t] = st;
+    }
+    return WHMEC_OK;
+}
+
+// whmec_genotype_batch: every table packed (a table that fails keeps its status and message), then groups of tables on one step
+// list each (gl_batch_groups under the budget work_budget applies), and every table that does not fit a group alone through the
+// single-table path.  A CUDA failure returns WHMEC_ERR_CUDA with `msg` (the caller reports it for every table).
+int genotype_batch_impl(const whmec_problem *const *problems, double *const *likelihoods, uint32_t n_tables, int device, int *status, char *errs,
+                        size_t errlen, whmec_stats *stats, whmec_stats &total, std::string &msg) {
+    auto err_of = [&](uint32_t t) { return errs ? errs + (size_t)t * errlen : nullptr; };
+    std::vector<Packed> pks(n_tables);
+    std::vector<GlPacked> gs(n_tables);
+    std::vector<uint64_t> cost(n_tables, 0);  // 0: not on the device (an error, or no columns)
+    bool any = false;
+    for (uint32_t t = 0; t < n_tables; ++t) {
+        status[t] = WHMEC_OK;
+        if (stats) stats[t] = whmec_stats{};
+        std::string m;
+        int rc = WHMEC_ERR_INPUT;
+        if (!problems[t] || !likelihoods[t]) m = "null argument";
+        else {
+            try {
+                rc = gl_pack(problems[t], pks[t], gs[t], m);
+            } catch (const std::exception &e) {
+                m = e.what();
+                rc = WHMEC_ERR_INPUT;
+            }
+        }
+        if (rc != WHMEC_OK) {
+            status[t] = rc;
+            set_err(err_of(t), errlen, m);
+            pks[t] = Packed();
+            gs[t] = GlPacked();
+            continue;
+        }
+        if (stats) stats[t] = pks[t].stats;
+        if (pks[t].n == 0) continue;
+        any = true;
+    }
+    if (!any) return WHMEC_OK;
+    int rc = open_device(device, msg);
+    if (rc != WHMEC_OK) return rc;
+    Buffers S;
+    CUDA_TRY(cudaStreamCreateWithFlags(&S.stream, cudaStreamNonBlocking));
+    const size_t free_b = device_available_bytes();
+    const uint64_t reserve = 512ull << 20;
+    uint64_t budget = free_b > reserve ? (free_b - reserve) / 8 : 0;
+    if (const char *e = std::getenv("WHMEC_GENOTYPE_ARENA_BUDGET")) budget = std::min<uint64_t>(budget, std::strtoull(e, nullptr, 10) / 8);
+    for (uint32_t t = 0; t < n_tables; ++t)
+        if (status[t] == WHMEC_OK && pks[t].n > 0) cost[t] = gl_batch_cost(pks[t], gs[t]);
+    std::vector<std::vector<uint32_t>> groups;
+    std::vector<uint32_t> alone;
+    gl_batch_groups(cost, budget, groups, alone);
+    for (const std::vector<uint32_t> &members : groups) {
+        GlBatchGroup gp;
+        gl_batch_plan(pks, gs, members, gp);
+        rc = run_batch_group(S.stream, gp, pks, gs, likelihoods, stats, total, msg);
+        if (rc != WHMEC_OK) return rc;
+        for (uint32_t t : members) {
+            pks[t] = Packed();
+            gs[t] = GlPacked();
+        }
+    }
+    for (uint32_t t : alone) {  // packed again there; its result, code and text are whmec_genotype's
+        pks[t] = Packed();
+        gs[t] = GlPacked();
+        whmec_stats st{};
+        std::string m;
+        try {
+            rc = genotype_impl(problems[t], likelihoods[t], device, &st, m);
+        } catch (const std::exception &e) {
+            m = e.what();
+            rc = WHMEC_ERR_INPUT;
+        }
+        if (rc == WHMEC_ERR_CUDA) {
+            msg = m;
+            return rc;
+        }
+        status[t] = rc;
+        set_err(err_of(t), errlen, m);
+        if (rc != WHMEC_OK) continue;
+        add_stats(total, st);
+        st.sweep_ms = st.h2d_ms = st.d2h_ms = 0;
+        if (stats) stats[t] = st;
+    }
+    return WHMEC_OK;
+}
+
 }  // namespace
 
 // A segment of a pedigree table on one device (include/whmec.h): packed and uploaded once, then the transfer pass and the run.
@@ -403,6 +633,31 @@ struct whmec_gl_segment {
 
 extern "C" int whmec_genotype(const whmec_problem *p, double *likelihoods, int device, whmec_stats *st, char *err, size_t errlen) {
     return guarded([&](std::string &msg) { return genotype_impl(p, likelihoods, device, st, msg); }, err, errlen);
+}
+
+extern "C" int whmec_genotype_batch(const whmec_problem *const *problems, double *const *likelihoods, uint32_t n_tables, int device, int *status,
+                                    char *errs, size_t errlen, whmec_stats *stats, whmec_stats *total) {
+    if (total) *total = whmec_stats{};
+    if (n_tables == 0) return WHMEC_OK;
+    if (!problems || !likelihoods || !status) return WHMEC_ERR_INPUT;
+    whmec_stats sum{};
+    std::string msg;
+    int rc;
+    try {
+        rc = genotype_batch_impl(problems, likelihoods, n_tables, device, status, errs, errlen, stats, sum, msg);
+    } catch (const std::exception &e) {  // out of host memory: the call failed
+        msg = e.what();
+        rc = WHMEC_ERR_UNSUPPORTED;
+    }
+    if (rc != WHMEC_OK) {  // the call failed: every table reports why
+        for (uint32_t t = 0; t < n_tables; ++t) {
+            status[t] = rc;
+            set_err(errs ? errs + (size_t)t * errlen : nullptr, errlen, msg);
+        }
+        return rc;
+    }
+    if (total) *total = sum;
+    return WHMEC_OK;
 }
 
 extern "C" int whmec_genotype_segment_create(const whmec_problem *p, int device, int continues, int continued, whmec_gl_segment **out, char *err,

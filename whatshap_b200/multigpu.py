@@ -827,15 +827,10 @@ def genotype_table(prob: FlatProblem, device: int = 0, devices: Optional[Sequenc
     return _lib.genotype(prob, device=device) if chosen is None else genotype_on_devices(prob, chosen)
 
 
-def solve_tables(problems: Sequence[FlatProblem], device: int = 0, devices: Optional[Sequence[int]] = None, with_stats: bool = False):
-    """Several tables at once: per table, in input order, its `FlatSolution` or the exception `solve_table` would have raised
-    for it (an input error, a Mendelian conflict, a refusal; a failure of the device raises, whatever the length of the list).
-    On one device this is `_lib.solve_batch` (tables share the GPU's sweeps).  With `devices` / WHMEC_DEVICES whole tables go
-    to devices by longest-processing-time-first on their DP cells sum 2^a * T (`block_work`, `assign_blocks`), one
-    `whmec_solve_batch` per device on that device's host thread.  A single table behaves like `solve_table`, including being
-    spread over the devices.  `with_stats`: (results, per-table stats) instead."""
-    from . import _lib
-
+def _tables(problems: Sequence[FlatProblem], device: int, devices: Optional[Sequence[int]], with_stats: bool, batch, single, weight):
+    """The driver of `solve_tables` and `genotype_tables`: `batch(problems, device)` -> (results, (per-table stats, totals)) runs
+    a list on one device, `single(problem, device, devices)` -> (result, stats) one table over several devices, and
+    `weight(problem)` is the work by which whole tables go to devices (longest-processing-time-first, `assign_blocks`)."""
     problems = list(problems)
     chosen = table_devices(device, devices)
     distinct = sorted(set(chosen)) if chosen is not None else [device]
@@ -843,18 +838,16 @@ def solve_tables(problems: Sequence[FlatProblem], device: int = 0, devices: Opti
     stats: list = [{} for _ in problems]
     if len(problems) == 1 and len(distinct) > 1:
         try:
-            out[0], stats[0] = solve_table(problems[0], device, devices)
+            out[0], stats[0] = single(problems[0], device, devices)
         except RuntimeError as e:  # MendelianConflict, input errors, Unsupported: the table's result
             if str(e).startswith("CUDA failure"):
                 raise
             out[0] = e
     elif len(distinct) == 1 or not problems:
-        out, (stats, _) = _lib.solve_batch(problems, device=distinct[0], with_stats=True)
+        out, (stats, _) = batch(problems, distinct[0])
     else:
-        work = np.array([float(block_work(p, [(0, p.n_cols)])[0]) * 4.0 ** p.n_trios for p in problems])
-        shares = assign_blocks(work, len(distinct))
-        jobs = [(lambda ids=ids, d=d: _lib.solve_batch([problems[i] for i in ids], device=d, with_stats=True)) if ids else None
-                for ids, d in zip(shares, distinct)]
+        shares = assign_blocks(np.array([weight(p) for p in problems]), len(distinct))
+        jobs = [(lambda ids=ids, d=d: batch([problems[i] for i in ids], d)) if ids else None for ids, d in zip(shares, distinct)]
         results, errors = _run_on_devices(distinct, jobs)
         for e in errors:
             if e is not None:
@@ -864,6 +857,60 @@ def solve_tables(problems: Sequence[FlatProblem], device: int = 0, devices: Opti
                 for i, r, st in zip(ids, res[0], res[1][0]):
                     out[i], stats[i] = r, st
     return (out, stats) if with_stats else out
+
+
+def solve_tables(problems: Sequence[FlatProblem], device: int = 0, devices: Optional[Sequence[int]] = None, with_stats: bool = False):
+    """Several tables at once: per table, in input order, its `FlatSolution` or the exception `solve_table` would have raised
+    for it (an input error, a Mendelian conflict, a refusal; a failure of the device raises, whatever the length of the list).
+    On one device this is `_lib.solve_batch` (tables share the GPU's sweeps).  With `devices` / WHMEC_DEVICES whole tables go
+    to devices by longest-processing-time-first on their DP cells sum 2^a * T (`block_work`, `assign_blocks`), one
+    `whmec_solve_batch` per device on that device's host thread.  A single table behaves like `solve_table`, including being
+    spread over the devices.  `with_stats`: (results, per-table stats) instead."""
+    from . import _lib
+
+    return _tables(problems, device, devices, with_stats, lambda ps, d: _lib.solve_batch(ps, device=d, with_stats=True),
+                   lambda p, dev, devs: solve_table(p, dev, devs),
+                   lambda p: float(block_work(p, [(0, p.n_cols)])[0]) * 4.0 ** p.n_trios)
+
+
+def genotype_tables(problems: Sequence[FlatProblem], device: int = 0, devices: Optional[Sequence[int]] = None, with_stats: bool = False):
+    """Several genotyping tables at once: per table, in input order, its likelihoods [n_ind, n_cols, 3] or the exception
+    `genotype_table` would have raised for it (a failure of the device raises, whatever the length of the list).  On one device
+    this is `_lib.genotype_batch` (tables share the GPU's launches).  With `devices` / WHMEC_DEVICES whole tables go to devices
+    by longest-processing-time-first on sum 2^a * T * 2^P (`block_work`, `assign_blocks`), one `whmec_genotype_batch` per
+    device on that device's host thread.  A single table behaves like `genotype_table`, including being spread over the
+    devices.  `with_stats`: (results, per-table stats) instead."""
+    from . import _lib
+
+    return _tables(problems, device, devices, with_stats, lambda ps, d: _lib.genotype_batch(ps, device=d, with_stats=True),
+                   lambda p, dev, devs: genotype_table(p, dev, devs),
+                   lambda p: float(block_work(p, [(0, p.n_cols)])[0]) * 4.0 ** p.n_trios * 2.0 ** (2 * (p.n_ind - p.n_trios)))
+
+
+def batch_objects(cls, tables, build, run, attr: str, return_exceptions: bool) -> list:
+    """The `batch` classmethods of the table classes: one `cls` object per constructor argument tuple of `tables`
+    (`build(obj, args)` fills it; an exception it raises takes the table's place), `run(problems)` -> (results, per-table stats or
+    None) over the `_problem` of every built object, each result stored in the object's `attr` (and its stats in `stats`) or,
+    when it is an exception, in the table's place.  Then `finish_batch`."""
+    objs: list = []
+    for args in tables:
+        try:
+            obj = cls.__new__(cls)
+            build(obj, args)
+            objs.append(obj)
+        except Exception as e:  # noqa: BLE001 - reported in the table's place, after the others ran
+            objs.append(e)
+    good = [i for i, o in enumerate(objs) if not isinstance(o, BaseException)]
+    results, stats = run([objs[i]._problem for i in good])
+    for n, (i, res) in enumerate(zip(good, results)):
+        if isinstance(res, BaseException):
+            objs[i] = res
+        else:
+            setattr(objs[i], attr, res)
+            if stats is not None:
+                objs[i].stats = stats[n]  # (times are 0: the tables shared their launches)
+    finish_batch(objs, return_exceptions)
+    return objs
 
 
 def finish_batch(results: list, return_exceptions: bool) -> None:
