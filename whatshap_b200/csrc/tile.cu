@@ -55,6 +55,7 @@ struct TileSmem {
     int32_t T5s[TC_CHUNK][32];
     uint32_t cgs[TC_CHUNK];
     SteadyCol scs[TC_CHUNK];            // steady-state panels: the per-column constants of column_fast, 32 bytes each
+    NarrowCol ncs[TC_CHUNK][2];         // narrow panels: the per-column constants of narrow_column_body, per parity of a thread's outputs
     unsigned long long bp_at[TC_CHUNK]; // steady-state panels: first back-pointer word of this tile in column j (bp_off + tile * stride)
     Panel P;
     uint32_t cg[2];
@@ -301,6 +302,68 @@ __device__ __forceinline__ void steady_columns(TileSmem &S, uint32_t ncol, uint3
 #endif
         col_phase ^= 1u;
     }
+}
+
+// Narrow steady-state panel (Panel::narrow): the columns of steady_columns<3, false> on halfword pairs (tile_fast.h:
+// narrow_column_body).  The tile's input moves into halfwords h = 2 (v - base), base = in[0] - Panel::narrow_spread, in the
+// other buffer of the ping-pong pair before the first column, and back into 32-bit values after the last one.
+__device__ __forceinline__ void steady_columns_narrow(TileSmem &S, uint32_t ncol, uint32_t spread, uint32_t *__restrict__ arena, uint32_t &cur,
+                                                      uint32_t &col_phase, uint32_t tid) {
+    const uint32_t lane = tid & 31u, warp = tid >> 5;
+    const uint32_t base = S.buf[cur][0] - spread;
+    {
+        const uint4 *src = reinterpret_cast<const uint4 *>(S.buf[cur]);
+        uint2 *dst = reinterpret_cast<uint2 *>(S.buf[cur ^ 1]);
+#pragma unroll
+        for (uint32_t i = tid; i < TILE_ENTRIES / 4; i += NT) {
+            const uint4 v = src[i];
+            dst[i] = make_uint2(((v.x - base) << 1) | ((v.y - base) << 17), ((v.z - base) << 1) | ((v.w - base) << 17));
+        }
+    }
+    if (tid < 2 * ncol) S.ncs[tid >> 1][tid & 1u] = narrow_col(S.tcs[tid >> 1], S.cgs[tid >> 1], tid & 1u);
+    cur ^= 1;
+    __syncthreads();
+    // constants of the panel: the thread's first word, the parity of its output bits (which NarrowCol record it reads)
+    const uint32_t word0 = warp * 128u + lane;
+    const uint32_t pp = (popc32(warp) + popc32(lane)) & 1u;
+    const uint32_t bp_word = warp * 16u + (lane & 15u);
+    NarrowPrep pr;
+    narrow_prep(pr, &S.ncs[0][pp], (uint32_t)(S.TWs[0][warp] + S.T5s[0][lane]), S.buf[cur], S.buf[cur ^ 1], word0);
+    uint32_t *bpw = arena + S.bp_at[0];
+    for (uint32_t j = 0; j < ncol; ++j) {
+        const uint32_t bits = narrow_column_body(pr);
+        const uint32_t other = __shfl_down_sync(0xFFFFFFFFu, bits, 16);
+        if (lane < 16) bpw[bp_word] = narrow_bp_word(bits, other);
+#if WHMEC_COL_ARRIVE_ALL
+        mbar_arrive(&S.col_bar);
+#else
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&S.col_bar);
+#endif
+        cur ^= 1;
+        if (j + 1 < ncol) {
+            narrow_prep(pr, &S.ncs[j + 1][pp], (uint32_t)(S.TWs[j + 1][warp] + S.T5s[j + 1][lane]), S.buf[cur], S.buf[cur ^ 1], word0);
+            bpw = arena + S.bp_at[j + 1];
+        }
+#ifdef WHMEC_TILE_PHASE_CLOCKS
+        const long long w0 = clock64();
+        mbar_wait(&S.col_bar, col_phase);
+        if (tid == 0) S.phase_wait += clock64() - w0;
+#else
+        mbar_wait(&S.col_bar, col_phase);
+#endif
+        col_phase ^= 1u;
+    }
+    {  // (the write-back starts with a barrier)
+        const uint2 *src = reinterpret_cast<const uint2 *>(S.buf[cur]);
+        uint4 *dst = reinterpret_cast<uint4 *>(S.buf[cur ^ 1]);
+#pragma unroll
+        for (uint32_t i = tid; i < TILE_ENTRIES / 4; i += NT) {
+            const uint2 h = src[i];
+            dst[i] = make_uint4(base + ((h.x & 0xFFFFu) >> 1), base + (h.x >> 17), base + ((h.y & 0xFFFFu) >> 1), base + (h.y >> 17));
+        }
+    }
+    cur ^= 1;
 }
 
 // Bulk version of stage_tile_async (called by warp 0 only): chunk tA lands at stage + tA * (2^j + BULK_SKEW), in the
@@ -561,6 +624,7 @@ tile_panel_kernel(const Panel *__restrict__ panels, const TileLaunch L, const Ti
             const uint32_t j = tid >> 6, idx = tid & 63u;
             if (j < ncol) {
                 if (idx < 32) S.TWs[j][idx] = tile_fast_warp_entry(S.tcs[j], tile, idx);
+                else if (P.narrow) S.T5s[j][idx - 32] = narrow_lane_entry(S.tcs[j], idx - 32);
                 else S.T5s[j][idx - 32] = tile_fast_lane_entry(S.tcs[j], idx - 32);
                 if (idx == 63) {
                     const uint32_t cg = tile_cg(S.tcs[j], tile);
@@ -574,7 +638,9 @@ tile_panel_kernel(const Panel *__restrict__ panels, const TileLaunch L, const Ti
         const uint32_t lg = P.steady - 1u;
         __syncthreads();  // tables ready; the tile's input is in place
         WHMEC_PHASE(2);
-        if (lg == 3) {
+        if (P.narrow) {
+            steady_columns_narrow(S, ncol, P.narrow_spread, arena, cur, col_phase, tid);
+        } else if (lg == 3) {
             if (mirror) steady_columns<3, true>(S, ncol, arena, cur, col_phase, tid);
             else steady_columns<3, false>(S, ncol, arena, cur, col_phase, tid);
         } else {

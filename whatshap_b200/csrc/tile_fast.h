@@ -196,6 +196,153 @@ WHMEC_HD void steady_prep(FastPrep<LG> &pr, const SteadyCol &sc, int32_t tw, int
     for (int it = 1; it < IT; ++it) pr.ue[it] = pr.ue[it & (it - 1)] + (uint32_t)sc.w[cx_ctz(it)];
 }
 
+// ---- narrow steady-state columns (Panel::narrow, DESIGN §4.1) ---------------------------------------------------------------
+// A narrow panel keeps its projection as 16-bit halfwords h = 2 (v - base) (one base per tile and panel), two per 32-bit word,
+// and a word is worked on as a pair of halves: Hopper's DPX instructions add and compare both halves at once
+// (VIADDMNMX.U16x2, VIMNMX.U16x2).  Every half stays inside [0, 2^16) (the planner's bound), so a plain 32-bit add of two
+// such pairs, read as lo + 65536 * hi with signed halves, is exact in both halves as well.
+//
+// Keys.  Candidate c of an output gets the key 2 (v_c + cost_c) + (c == the candidate the reference visits second): the
+// minimum of the two keys is 2 * the output's value plus the output's back-pointer bit (pick1 ^ par, the bit the u32 path
+// stores); the keys never tie (their low bits differ).
+//
+// Thread mapping (2^14 outputs, 1024 threads, 16 outputs each).  A word holds outputs o and o + 1 (the halves of the same
+// words in the next column are again its candidates: the layout of the halfword array does not change from column to
+// column).  Thread (warp w, lane L) owns the words of the outputs  w * 256 + iq * 64 + 2 L + {0, 1}  (iq = 0..3) and their
+// twins (+ 2^13): the halfwords 4 (w * 128 + iq * 32 + L) .. + 3 of the input are the candidates of both words of a
+// quad, one 64-bit load.  The back-pointer element of thread-packed lane l (16 bits, tile_packed_bit_index) holds outputs
+// with lane bits l, so lane L produces half of the elements of lanes 2 (L & 15) and 2 (L & 15) + 1, lane L ^ 16 the other
+// half: one shuffle joins them, and the lanes L < 16 store both elements as one 32-bit word.
+constexpr uint32_t NARROW_TWIN_WORDS = 1u << 12;  // words between an output pair and its twins (2^13 outputs)
+
+WHMEC_HD uint32_t narrow_vmin2(uint32_t a, uint32_t b) {  // per-half unsigned min: VIMNMX.U16x2
+#if defined(__CUDA_ARCH__)
+    return __vminu2(a, b);
+#else
+    const uint32_t lo = (a & 0xFFFFu) < (b & 0xFFFFu) ? (a & 0xFFFFu) : (b & 0xFFFFu);
+    const uint32_t hi = (a >> 16) < (b >> 16) ? (a >> 16) : (b >> 16);
+    return lo | (hi << 16);
+#endif
+}
+
+WHMEC_HD uint32_t narrow_viaddmin2(uint32_t a, uint32_t b, uint32_t c) {  // per half min(a + b mod 2^16, c): VIADDMNMX.U16x2
+#if defined(__CUDA_ARCH__)
+    return __viaddmin_u16x2(a, b, c);
+#else
+    return narrow_vmin2(((a + b) & 0xFFFFu) | (((a >> 16) + (b >> 16)) << 16), c);
+#endif
+}
+
+WHMEC_HD uint32_t narrow_prmt(uint32_t a, uint32_t b, uint32_t sel) {  // PRMT: byte i of the result = byte sel_i of (b:a)
+#if defined(__CUDA_ARCH__)
+    return __byte_perm(a, b, sel);
+#else
+    const uint64_t ab = ((uint64_t)b << 32) | a;
+    uint32_t r = 0;
+    for (uint32_t i = 0; i < 4; ++i) r |= (uint32_t)((ab >> (8 * ((sel >> (4 * i)) & 7u))) & 0xFFu) << (8 * i);
+    return r;
+#endif
+}
+
+// The constants of one narrow column for the threads whose output bits have parity p (with the column's cg: the tie-break
+// parity par of their first output), built once per (tile, column, p) next to the steady-state tables.
+// Candidate roles: the VIADDMNMX below adds 4 |wp| (wp = weight of the read that ends) to the cost pair of one candidate,
+// which must not wrap; with wp < 0 the roles of the two candidates swap (the "first" candidate is candidate 1: its U is
+// U + wp, its parity 1 - par, and the PRMT selectors exchange the candidates' values).  Below, U and par are those of the
+// first candidate.
+// Word (iq, twin) of a thread starts from  a = 2 U + par  per half (par of the high half = 1 - par of the low one);
+// a[0] = u * 131074 + a0c with u the thread's U of output 2L, a[i] = a[0] + d[i].  With f = parity(iq) ^ twin,
+// kp[f] - a = 2 (K12 - U) + par per half, and  min(2 U' + 1 - par, 2 (K12 - U') + 1 - par)  of the other candidate
+// (U' = U + |wp|) = viaddmin(a, w4, kp[f] - a) + dy[f].
+struct alignas(16) NarrowCol {
+    uint32_t a0c;
+    uint32_t d[7];
+    uint32_t kp[2], dy[2];
+    uint32_t w4, selx, sely, pad;
+};
+
+WHMEC_HD NarrowCol narrow_col(const TileCol &tc, uint32_t cg, uint32_t p) {
+    NarrowCol nc;
+    const bool neg = tc.w_local[0] < 0;
+    const uint32_t awp = (uint32_t)(neg ? -tc.w_local[0] : tc.w_local[0]);
+    const uint32_t q = (p ^ cg ^ (neg ? 1u : 0u)) & 1u;  // par of the first candidate of the low half of word 0
+    const uint32_t G = q ? 65535u : (uint32_t)-65535;    // a(f = 1) - a(f = 0) at equal U
+    const uint32_t d6 = (uint32_t)tc.w_local[7] * 131074u, d7 = (uint32_t)tc.w_local[8] * 131074u;
+    const uint32_t dn = (uint32_t)tc.w_local[tc.l_out] * 131074u;
+    nc.a0c = ((uint32_t)tc.w_local[1] << 17) + (q ? 1u : 65536u);
+    nc.d[0] = dn + G;            // (iq 0, twin)
+    nc.d[1] = d6 + G;            // (iq 1)
+    nc.d[2] = d6 + dn;           // (iq 1, twin)
+    nc.d[3] = d7 + G;            // (iq 2)
+    nc.d[4] = d7 + dn;           // (iq 2, twin)
+    nc.d[5] = d6 + d7;           // (iq 3)
+    nc.d[6] = d6 + d7 + dn + G;  // (iq 3, twin)
+    nc.kp[0] = tc.K12 * 131074u + (q ? 2u : 131072u);
+    nc.kp[1] = nc.kp[0] + 2u * G;
+    nc.dy[0] = G - awp * 131074u;
+    nc.dy[1] = (0u - G) - awp * 131074u;
+    nc.w4 = awp * 262148u;
+    nc.selx = neg ? 0x7632u : 0x5410u;  // halves 0 / 1 of the two words of a quad: candidate 0 / 1
+    nc.sely = neg ? 0x5410u : 0x7632u;
+    nc.pad = 0;
+    return nc;
+}
+
+// Narrow lane table: U of output 2L of lane L (output bits 1..5; the warp table adds K2, the global reads and bits 8..12),
+// plus wp when candidate 1 is the first one.
+WHMEC_HD int32_t narrow_lane_entry(const TileCol &tc, uint32_t lane) {
+    int32_t s = tile_fast_lane_entry(tc, (2u * lane) & 31u);
+    if (lane >> 4) s += tc.w_local[6];
+    if (tc.w_local[0] < 0) s += tc.w_local[0];
+    return s;
+}
+
+// What a thread carries of one narrow column across the column barrier (like FastPrep, but small: the record is read by the
+// body, so that the thread's registers are not tied up while it waits).
+struct NarrowPrep {
+    const TilePair *sin;    // this thread's first candidate quad
+    uint32_t *so;           // this thread's first output word
+    const NarrowCol *nc;    // the column's record for the parity of the thread's outputs
+    uint32_t a0;
+};
+
+WHMEC_HD void narrow_prep(NarrowPrep &pr, const NarrowCol *nc, uint32_t u, const uint32_t *__restrict__ Hin, uint32_t *__restrict__ Hout,
+                          uint32_t word0) {
+    pr.sin = reinterpret_cast<const TilePair *>(Hin) + word0;
+    pr.so = Hout + word0;
+    pr.nc = nc;
+    pr.a0 = u * 131074u + nc->a0c;
+}
+
+// One narrow column of one thread: stores its 8 output words, returns its 16 back-pointer bits (bits of outputs 2L + 0 in the
+// low half, 2L + 1 in the high half, at the element positions of lane group L & 16 == 0; narrow_bp_word places them).
+WHMEC_HD uint32_t narrow_column_body(const NarrowPrep &pr) {
+    const NarrowCol nc = *pr.nc;
+    uint32_t bits = 0;
+#pragma unroll
+    for (int iq = 0; iq < 4; ++iq) {
+        const TilePair s = pr.sin[iq * 32];
+        const uint32_t x = narrow_prmt(s.x, s.y, nc.selx);  // first candidate of outputs 2L, 2L + 1
+        const uint32_t y = narrow_prmt(s.x, s.y, nc.sely);  // the other candidate
+#pragma unroll
+        for (int tw = 0; tw < 2; ++tw) {
+            const int f = (int)(cx_parity(iq) ^ tw);
+            const uint32_t a = (iq == 0 && tw == 0) ? pr.a0 : pr.a0 + nc.d[2 * iq + tw - 1];
+            const uint32_t c0 = narrow_vmin2(a, nc.kp[f] - a);
+            const uint32_t c1 = narrow_viaddmin2(a, nc.w4, nc.kp[f] - a);
+            const uint32_t m = narrow_vmin2(x + c0, y + c1 + nc.dy[f]);
+            pr.so[iq * 32 + tw * NARROW_TWIN_WORDS] = m & 0xFFFEFFFEu;
+            // element bit 15 - 4 iq - tw (lane group 0); the shifts between consecutive outputs are 1 and 3
+            bits = (iq == 0 && tw == 0) ? (m & 0x10001u) : (bits << (tw ? 1 : 3)) + (m & 0x10001u);
+        }
+    }
+    return bits;
+}
+
+// The 32-bit word that lane L (< 16) of a warp stores: its bits and those of lane L + 16 (bits of the lane group 1, two
+// element positions lower).
+WHMEC_HD uint32_t narrow_bp_word(uint32_t bits_lo_group, uint32_t bits_hi_group) { return (bits_lo_group << 2) | bits_hi_group; }
+
 template <int LG, bool HASK0, bool SHARE, bool PACKED = false, bool MIRROR = false, class Emit>
 WHMEC_HD void column_fast(const TileCol &tc, const int32_t *__restrict__ TW, const int32_t *__restrict__ T5,
                           uint32_t cg, const uint32_t *__restrict__ Sin, uint32_t *__restrict__ Sout, Emit emit, uint32_t tid) {

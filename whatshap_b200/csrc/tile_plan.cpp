@@ -32,6 +32,8 @@ void plan_tiles(const Packed &pk, TileSchedule &ts) {
     const bool packed_bp = !(packed_env && packed_env[0] == '0');  // the default; "0" keeps the warp-ballot layout
     const char *mirror_env = std::getenv("WHMEC_TILE_MIRROR");
     const bool mirror_on = !(mirror_env && mirror_env[0] == '0');  // "0": every tile of every panel is computed (test hook)
+    const char *narrow_env = std::getenv("WHMEC_TILE_NARROW");
+    const bool narrow_on = !(narrow_env && narrow_env[0] == '0');  // "0": steady panels keep the 32-bit columns (test hook)
     auto tnow = [] { return std::chrono::steady_clock::now(); };
     auto tms = [](std::chrono::steady_clock::time_point a, std::chrono::steady_clock::time_point b) { return std::chrono::duration<double, std::milli>(b - a).count(); };
     const auto t0 = tnow();
@@ -79,6 +81,9 @@ void plan_tiles(const Packed &pk, TileSchedule &ts) {
         chain_state_words[c] = 2 * buf_words;
         uint64_t bp_words = 0;
         uint32_t pcount = 0;
+        // narrow panels: sum of |weight| of every read over the columns [k0, cum_col)
+        std::vector<uint64_t> cum_w(narrow_on ? nr : 0, 0);
+        uint32_t cum_col = k0;
 
         Small state;  // reads kept after column k-1, canonical (ascending) order
         uint32_t k = k0;
@@ -334,6 +339,32 @@ void plan_tiles(const Packed &pk, TileSchedule &ts) {
                                  tc.l_in == t0.l_in && tc.l_out == t0.l_out && (tc.half && tc.km != 0) == (t0.half && t0.km != 0);
                     }
                     P.steady = steady ? 1u + t0.pad1 : 0u;
+                    // Narrow (16-bit) sweep of a steady panel with 2^14-entry tiles, whose values provably stay inside
+                    // TILE_NARROW_LIMIT (DESIGN §4.1).  The input spread: two entries of one tile differ only in the tile's
+                    // local reads Lold; flipping them moves every earlier column's cost by at most their |weights| there.
+                    const bool plain = !(t0.half && t0.km != 0) && t0.l_in == TILE_SMAX && t0.l_out == TILE_SMAX;
+                    if (narrow_on && P.steady == 4 && plain) {
+                        for (; cum_col < k; ++cum_col) {  // |weights| of every read up to column k - 1
+                            const ColMeta &m = pk.cols[cum_col];
+                            const uint32_t *reads = col_reads(pk, cum_col);
+                            const uint8_t *al = pk.act_allele.data() + pk.act_off[cum_col];
+                            const uint32_t *ph = pk.act_phred.data() + pk.act_off[cum_col];
+                            for (uint32_t q = 0; q < m.a; ++q)
+                                if (al[q] <= 1) cum_w[reads[q] - rbase] += ph[q];
+                        }
+                        uint64_t spread = 0;
+                        for (uint32_t q = 0; q < Lold.n; ++q) spread += cum_w[Lold.v[q] - rbase];
+                        bool fits = spread < TILE_NARROW_LIMIT;
+                        for (uint32_t q = k; q < j && fits; ++q) {  // cost keys of a column: 2 K12 + 4 |wp| + 1 < 2^16
+                            const TileCol &tc = ts.cols[q];
+                            const uint64_t awp = (uint64_t)std::abs((int64_t)tc.w_local[0]);
+                            fits = 2ull * tc.K12 + 4ull * awp + 2ull <= 2ull * TILE_NARROW_LIMIT;
+                        }
+                        if (fits && narrow_panel_bound((uint32_t)spread, &ts.cols[k], j - k) < TILE_NARROW_LIMIT) {
+                            P.narrow = 1;
+                            P.narrow_spread = (uint32_t)spread;
+                        }
+                    }
                 }
                 per_chain[c].push_back(P);
                 per_chain_sets[c].push_back(PanelSets{G, Lcur, Lold, Gold});

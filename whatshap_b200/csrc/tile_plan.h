@@ -29,6 +29,7 @@ constexpr uint32_t TILE_MMAX = WHMEC_TILE_SMAX + 1;  // log2 cells a tile evalua
 constexpr uint32_t TILE_GMAX = 18;   // log2 tiles per panel (32 active reads = 14 local + 18 global)
 constexpr uint32_t TILE_KINF = 1u << 30;
 constexpr uint64_t TILE_SAFE_BOUND = 1ull << 28;  // every real cost must stay below this
+constexpr uint32_t TILE_NARROW_LIMIT = 1u << 15;  // narrow panels: every value minus the tile's base, plus a cost, stays below this
 
 struct TileCol {            // one column as seen by a tile (device + host)
     uint8_t l_in, n_new, d, l_out;
@@ -84,6 +85,11 @@ struct Panel {
     // back-pointers, one mirror mode.  The kernel sweeps such a panel with all per-column tables built once, in
     // parallel, and no per-column dispatch.  steady = 1 + LG (2^LG twin pairs per thread), 0 otherwise.
     uint32_t steady;
+    // Narrow steady-state panel (2^14-entry tiles, not mirrored with km != 0): the kernel sweeps it on 16-bit halfword pairs
+    // (tile_fast.h), values relative to base = (the tile's first input entry) - narrow_spread.  narrow_spread bounds how far
+    // apart any two input entries of one tile are; with it, every value of the panel minus base stays below TILE_NARROW_LIMIT
+    // (the planner's proof: DESIGN §4.1).
+    uint32_t narrow, narrow_spread;
     // The previous panel of the chain (index into TileSchedule::panels; TILE_NO_PANEL for a fresh panel), whose output is this
     // panel's input, and its number of computed tiles: the kernel starts a tile of this panel once that many tiles of the
     // producer have signalled their write-back.
@@ -91,6 +97,14 @@ struct Panel {
     uint64_t in_off, out_off;      // 32-bit word offsets of the chain's state buffers
 };
 constexpr uint32_t TILE_NO_PANEL = 0xFFFFFFFFu;
+
+// Narrow panels: largest value minus the tile's base after the first `ncol` columns (DESIGN §4.1): twice the input spread
+// (base = first input entry - spread) plus, per column, the largest cell cost min(K2 + E, K1 - E) <= K12 / 2.
+inline uint64_t narrow_panel_bound(uint32_t spread, const TileCol *cols, uint32_t ncol) {
+    uint64_t b = 2ull * spread;
+    for (uint32_t j = 0; j < ncol; ++j) b += cols[j].K12 / 2;
+    return b;
+}
 inline uint32_t panel_tiles(const Panel &P) { return 1u << (P.g - P.half); }  // computed tiles (mirrored panel: half of 2^g)
 
 struct TileSchedule {
