@@ -104,7 +104,7 @@ typedef struct whmec_stats {
     float h2d_ms, d2h_ms;        /* device-timed copies of the last solve */
     uint64_t h2d_bytes, d2h_bytes;
     uint32_t path_kind;          /* 1 = tile kernel, 2 = column kernel, 3 = batched pedigree sweep, 4 = genotyping (forward-backward),
-                                    5 = wide column sweep (five trios, T = 1024) */
+                                    5 = wide column sweep (five trios, T = 1024), 6 = heuristic swept on the device */
     uint32_t reserved;
 } whmec_stats;
 
@@ -311,6 +311,24 @@ typedef struct whmec_heuristic_solution {
 } whmec_heuristic_solution;
 int whmec_heuristic(const whmec_problem *p, uint32_t row_limit, int allow_mutations, whmec_heuristic_solution *s, char *err,
                     size_t errlen);
+
+/* Many heuristic tables in one call (`whatshap phase --algorithm=heuristic` builds one PedMecHeuristic per chromosome x family;
+ * with a multi-sample VCF every sample is a table of its own).  solutions[t] receives, bit for bit, what
+ * whmec_heuristic(problems[t], row_limits[t], allow_mutations[t], ...) writes.  On the GPU one CTA sweeps one table, its partial
+ * solutions spread over the CTA's threads; tables are cut, longest first (columns x row_limit), into groups whose device memory
+ * fits the free HBM (or WHMEC_HEURISTIC_ARENA_BUDGET), one launch per group.  whmec_heuristic runs inside the call, with the
+ * same result, for: allow_mutations == 0, tables without reads, columns or samples, more than 16 samples, input errors, tables
+ * that fit no group alone, and tables whose partial solutions outgrow their device row buffers (ties at the optimum can keep
+ * any number of them).  Errors are per table: status[t] and the message at errs + t * errlen (errs may be NULL) are what
+ * whmec_heuristic returns for table t.  The return value is WHMEC_ERR_INPUT for null arguments, WHMEC_ERR_CUDA for a device
+ * failure (then every status holds it and every message the reason; running out of host memory fails the call the same way,
+ * with WHMEC_ERR_UNSUPPORTED), WHMEC_OK otherwise; n_tables == 0 does nothing.  stats (optional, [n_tables]): path_kind 6 for
+ * a table swept on the device (0: whmec_heuristic), cells = columns x row_limit, max_active, transmissions; total (optional):
+ * device time and launches of the call, bytes copied to and from the device. */
+int whmec_heuristic_batch(const whmec_problem *const *problems, whmec_heuristic_solution *const *solutions, const uint32_t *row_limits /* [n_tables] */,
+                          const int *allow_mutations /* [n_tables] */, uint32_t n_tables, int device, int *status /* [n_tables] */,
+                          char *errs /* [n_tables][errlen] or NULL */, size_t errlen, whmec_stats *stats_or_null /* [n_tables] */,
+                          whmec_stats *total_or_null);
 
 #ifdef __cplusplus
 }

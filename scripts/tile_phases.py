@@ -38,7 +38,8 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = os.path.join(ROOT, "whatshap_b200", "csrc")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
-OBJS = ["whmec.o", "genotype.o", "col_plan.o", "gl_batch.o", "gl_pack.o", "pack.o", "tile_plan.o", "hostpool.o", "readselect.o", "heuristic.o"]
+OBJS = ["whmec.o", "genotype.o", "col_plan.o", "gl_batch.o", "gl_pack.o", "pack.o", "tile_plan.o", "hostpool.o", "readselect.o", "heuristic.o",
+        "heuristic_batch.o", "heuristic_cu.o"]
 REC_WORDS = 8  # PhaseRec: t[5], wait, (smid, block), (steady, producer_wait)
 CAP = 1 << 20
 

@@ -50,6 +50,7 @@ EXPORTS = (
     "whmec_genotype_segment_destroy",
     "whmec_compute_genotypes",
     "whmec_heuristic",
+    "whmec_heuristic_batch",
 )
 
 
@@ -91,6 +92,10 @@ def lib() -> C.CDLL:
     L.whmec_compute_genotypes.restype = C.c_int
     L.whmec_heuristic.argtypes = [C.POINTER(CProblem), C.c_uint32, C.c_int, C.POINTER(CHeuristicSolution), C.c_char_p, C.c_size_t]
     L.whmec_heuristic.restype = C.c_int
+    L.whmec_heuristic_batch.argtypes = [C.POINTER(C.POINTER(CProblem)), C.POINTER(C.POINTER(CHeuristicSolution)), C.POINTER(C.c_uint32),
+                                        C.POINTER(C.c_int), C.c_uint32, C.c_int, C.POINTER(C.c_int), C.c_char_p, C.c_size_t, C.POINTER(CStats),
+                                        C.POINTER(CStats)]
+    L.whmec_heuristic_batch.restype = C.c_int
     L.whmec_read_sort_key.argtypes = [C.c_char_p, C.c_size_t, C.c_int32]
     L.whmec_read_sort_key.restype = C.c_uint64
     u32p = C.POINTER(C.c_uint32)
@@ -222,6 +227,62 @@ def heuristic(prob: FlatProblem, row_limit: int = 256, allow_mutations: bool = T
     raise_for(rc, err.value.decode())
     sol.score, sol.n_samples = float(cs.score), int(cs.n_samples)
     return sol
+
+
+def heuristic_arguments(problems: Sequence[FlatProblem], row_limits, allow_mutations):
+    """The ctypes arguments of `whmec_heuristic_batch` (and of its test emulation): (keep-alive objects, problems, solutions,
+    row limits, allow_mutations, status, errs, errlen, result objects).  `row_limits` / `allow_mutations`: one per table or one
+    for all."""
+    n = len(problems)
+    if isinstance(row_limits, (int, np.integer)):
+        row_limits = [row_limits] * n
+    if isinstance(allow_mutations, (bool, int, np.integer)):
+        allow_mutations = [allow_mutations] * n
+    row_limits, allow_mutations = list(row_limits), list(allow_mutations)
+    if len(row_limits) != n or len(allow_mutations) != n:
+        raise ValueError("row_limits and allow_mutations need one entry per table")
+    sols = [HeuristicSolution(p.n_cols, p.n_reads, p.n_ind) for p in problems]
+    cps, css = [p.as_c() for p in problems], [s.as_c() for s in sols]
+    pp = (C.POINTER(CProblem) * max(n, 1))(*[C.pointer(c) for c in cps])
+    sp = (C.POINTER(CHeuristicSolution) * max(n, 1))(*[C.pointer(c) for c in css])
+    rl = (C.c_uint32 * max(n, 1))(*[int(r) for r in row_limits])
+    am = (C.c_int * max(n, 1))(*[int(bool(a)) for a in allow_mutations])
+    status = (C.c_int * max(n, 1))()
+    errlen = 512
+    errs = C.create_string_buffer(errlen * max(n, 1))
+    return (cps, css), pp, sp, rl, am, status, errs, errlen, sols
+
+
+def heuristic_results(keep, status, errs, errlen, sols) -> list:
+    """Per table its `HeuristicSolution` or the exception `heuristic` raises for it (after `whmec_heuristic_batch`)."""
+    css = keep[1]
+    out: List[Union[HeuristicSolution, Exception]] = []
+    for t, sol in enumerate(sols):
+        try:
+            raise_for(int(status[t]), errs.raw[t * errlen:(t + 1) * errlen].split(b"\0", 1)[0].decode())
+            sol.score, sol.n_samples = float(css[t].score), int(css[t].n_samples)
+            out.append(sol)
+        except Exception as e:  # noqa: BLE001 - handed to the caller in the table's place
+            out.append(e)
+    return out
+
+
+def heuristic_batch(problems: Sequence[FlatProblem], row_limits=256, allow_mutations=True, device: int = 0, with_stats: bool = False):
+    """Several heuristic tables through one `whmec_heuristic_batch`: a list with, per table and in input order, its
+    `HeuristicSolution` -- bit for bit what `heuristic` gives for it alone -- or the exception `heuristic` would have raised for it
+    (the other tables are still solved).  `row_limits` / `allow_mutations`: per table, or one value for all.  A failure of the
+    call itself (no device, a CUDA error) raises.  `with_stats`: also returns (per-table stats, totals of the call)."""
+    keep, pp, sp, rl, am, status, errs, errlen, sols = heuristic_arguments(problems, row_limits, allow_mutations)
+    n = len(sols)
+    stats, total = (CStats * max(n, 1))(), CStats()
+    rc = lib().whmec_heuristic_batch(pp, sp, rl, am, n, device, status, errs, errlen, stats, C.byref(total))
+    if rc != 0:
+        message = errs.raw[:errlen].split(b"\0", 1)[0].decode() if n else ""
+        raise_for(rc, message or "whmec_heuristic_batch: invalid arguments")
+    out = heuristic_results(keep, status, errs, errlen, sols)
+    if with_stats:
+        return out, ([stats[t].as_dict() for t in range(n)], total.as_dict())
+    return out
 
 
 def compute_genotypes(prob: FlatProblem) -> Tuple[np.ndarray, np.ndarray]:

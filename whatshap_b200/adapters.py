@@ -276,14 +276,25 @@ def make_heuristic_class(core_module):
     class PedMecHeuristic:
         def __init__(self, readset, recombcost, pedigree, row_limit=256, distrust_genotypes=False, positions=None, allow_mutations=True,
                      verbosity=0):
+            self._setup(readset, recombcost, pedigree, distrust_genotypes, positions)
+            self._solution = _lib.heuristic(self._problem, min(max(int(row_limit), 0), 65535), bool(allow_mutations))
+
+        def _setup(self, readset, recombcost, pedigree, distrust_genotypes, positions):
             self.pedigree = pedigree
             # genotype likelihoods play no role in the heuristic: flatten with trusted genotypes, keep the flag for the solver
             self._problem, ids = flatten_objects(readset, recombcost, pedigree, False, positions)
             if list(ids) != list(range(len(ids))):
                 raise RuntimeError("PedMecHeuristic: sample ids must be the zero-based indices of the pedigree's individuals")
             self._problem.distrust = bool(distrust_genotypes)
-            self._solution = _lib.heuristic(self._problem, min(max(int(row_limit), 0), 65535), bool(allow_mutations))
             self._sample_ids = sorted(set(self._problem.read_ind.tolist()) | set(self._problem.trios.tolist()))
+
+        @classmethod
+        def batch(cls, tables, device=0, devices=None, return_exceptions=False):
+            """Several tables in one call (`core.PedMecHeuristic.batch`): `tables` holds constructor argument tuples."""
+            def setup(obj, args):
+                obj._setup(args[0], args[1], args[2], args[4] if len(args) > 4 else False, args[5] if len(args) > 5 else None)
+
+            return multigpu.batch_heuristic_objects(cls, tables, setup, device, devices, return_exceptions)
 
         def get_super_reads(self):
             prob, sol = self._problem, self._solution

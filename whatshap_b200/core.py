@@ -805,12 +805,18 @@ class PedigreeDPTable:
 class PedMecHeuristic:
     """Row-limited heuristic PedMEC solver, `whatshap phase --algorithm=heuristic` (core.pyx:674-734, src/pedmecheuristic.cpp).
 
-    Same constructor and methods as the reference binding.  Unlike `PedigreeDPTable` this is HOST code (`whmec_heuristic`,
-    csrc/heuristic.cpp): a sequential beam search over float scores whose results equal the reference's bit for bit.
+    Same constructor and methods as the reference binding.  Unlike `PedigreeDPTable` one table is HOST code (`whmec_heuristic`,
+    csrc/heuristic.cpp): a sequential beam search over float scores whose results equal the reference's bit for bit.  Many tables
+    go to the GPU together through `batch` (one CTA per table, the same results).
     The reads' sample ids must be the zero-based indices of the pedigree's individuals (src/pedmecheuristic.h:66)."""
 
     def __init__(self, readset: ReadSet, recombcost, pedigree: Pedigree, row_limit: int = 256, distrust_genotypes: bool = False,
                  positions=None, allow_mutations: bool = True, verbosity: int = 0):
+        self._setup(readset, recombcost, pedigree, distrust_genotypes, positions)
+        self._solution = _lib.heuristic(self._problem, min(max(int(row_limit), 0), 65535), bool(allow_mutations))
+
+    def _setup(self, readset, recombcost, pedigree, distrust_genotypes, positions) -> None:
+        """The constructor's checks and its flat problem (`_problem`), before the solver runs."""
         if not isinstance(readset, ReadSet):
             raise TypeError("Argument 'readset' has incorrect type")
         if not isinstance(pedigree, Pedigree):
@@ -840,9 +846,20 @@ class PedMecHeuristic:
             ent_allele=np.array(ent_allele, np.uint8), ent_phred=np.array(ent_phred, np.uint32), read_ind=np.array(read_ind, np.uint32),
             recombcost=np.array(rc[:n], np.uint32), n_ind=n_ind, trios=np.array([x for t in pedigree._triples for x in t], np.uint32),
             distrust=bool(distrust_genotypes), gt=gt, gl=None)
-        self._solution = _lib.heuristic(self._problem, min(max(int(row_limit), 0), 65535), bool(allow_mutations))
         # the samples the solver knows: ids of the reads and of the trio members, ascending (pedmecheuristic.cpp:52-63)
         self._sample_ids = sorted(set(self._problem.read_ind.tolist()) | set(self._problem.trios.tolist()))
+
+    @classmethod
+    def batch(cls, tables, device: int = 0, devices=None, return_exceptions: bool = False) -> list:
+        """Several tables in one call, one CTA of the GPU per table (`multigpu.heuristic_tables`, `whmec_heuristic_batch`).  `tables`
+        is a sequence of constructor argument tuples `(readset, recombcost, pedigree[, row_limit[, distrust_genotypes[, positions[,
+        allow_mutations[, verbosity]]]]])`; every returned object answers exactly like `cls(*arguments)`.  A table that fails does
+        not stop the others: afterwards the error of the lowest-index failing table is raised, with the type and text the
+        constructor would have raised; with `return_exceptions` the exception instance takes the table's place instead."""
+        def setup(obj, args):
+            obj._setup(args[0], args[1], args[2], args[4] if len(args) > 4 else False, args[5] if len(args) > 5 else None)
+
+        return multigpu.batch_heuristic_objects(cls, tables, setup, device, devices, return_exceptions)
 
     def get_super_reads(self) -> Tuple[List[ReadSet], List[int]]:
         """One ReadSet per sample with `superread_0` / `superread_1` (quality 30 everywhere, pedmecheuristic.cpp:104-117),

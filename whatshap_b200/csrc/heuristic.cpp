@@ -22,12 +22,14 @@
 #include <unordered_map>
 #include <vector>
 
-#include "../../include/whmec.h"
+#include "heuristic.h"
+
+using namespace whmec;
 
 namespace {
 
-using Score = float;  // MecScore (src/mecheader.h)
-constexpr uint32_t MAX_ROWS = 65535;  // MAX_ROW_LIMIT
+using Score = HeurScore;
+constexpr uint32_t MAX_ROWS = HEUR_MAX_ROWS;
 
 struct Partial {
     std::vector<uint8_t> side;    // side of every read that was active at the end of the previous column (kept reads first)
@@ -38,15 +40,8 @@ struct Partial {
     std::vector<Score> votes;     // [2 * S][W]: signed votes (positive: allele 1) per sample haplotype and window column
 };
 
-struct Solver {
-    const whmec_problem *p;
-    uint32_t n, m, S = 0, n_trios, tm_bits, row_limit, W = 1;
-    bool distrust, allow_mut;
-    std::vector<Score> rc, mc;             // recombination / mutation cost per column
-    std::vector<uint32_t> first, last;     // column span of every read
-    std::vector<uint32_t> sample_of_read;  // index into the sorted sample list
-    std::vector<uint32_t> trios;           // [3 * n_trios] as sample indices
-    std::vector<int> gt;                   // [S][n]  0 / 1 / 2
+struct Solver : HeurTable {
+    uint32_t row_limit, W = 1;
 
     Score &vote(Partial &q, uint32_t row, uint32_t i) const { return q.votes[(size_t)row * W + i]; }
     Score vote(const Partial &q, uint32_t row, uint32_t i) const { return q.votes[(size_t)row * W + i]; }
@@ -70,76 +65,6 @@ struct Solver {
                 }
             }
         return cost;
-    }
-
-    // best joint phasing of one column given the votes of all sample haplotypes (getOptPhasing, :462-560)
-    Score best_phasing(const std::vector<Score> &v, uint32_t t, uint32_t col, int8_t *alleles, uint8_t *mutated) const {
-        std::vector<Score> pc((size_t)S * 5);
-        for (uint32_t s = 0; s < S; ++s) {
-            const Score a0 = v[2 * s], a1 = v[2 * s + 1];
-            Score *c = &pc[(size_t)s * 5];
-            c[0] = (a0 * (a0 > 0) + a1 * (a1 > 0));
-            c[1] = (-a0 * (a0 < 0) + a1 * (a1 > 0));
-            c[2] = (a0 * (a0 > 0) - a1 * (a1 < 0));
-            c[3] = (-a0 * (a0 < 0) - a1 * (a1 < 0));
-            c[4] = *std::max_element(c, c + 4);
-        }
-        // allowed phasings per sample: 0 = 0|0, 1 = 0|1, 2 = 1|0, 3 = 1|1
-        std::vector<std::vector<int>> ph(S);
-        for (uint32_t s = 0; s < S; ++s) {
-            if (distrust) {
-                for (int i = 0; i < 4; ++i)
-                    if (pc[(size_t)s * 5 + i] < pc[(size_t)s * 5 + 4] + 2 * mc[col]) ph[s].push_back(i);
-            } else {
-                const int g = gt[(size_t)s * n + col];
-                if (g == 0) ph[s].push_back(0);
-                else if (g == 2) ph[s].push_back(3);
-                else {
-                    ph[s].push_back(1);
-                    ph[s].push_back(2);
-                }
-            }
-        }
-        Score best = std::numeric_limits<Score>::infinity();
-        // (a sample without any allowed phasing -- possible with distrusted genotypes where the mutation cost is 0 -- makes the
-        //  reference index an empty vector, :505-530; here such a column has no finite phasing)
-        for (uint32_t s = 0; s < S; ++s)
-            if (ph[s].empty()) return best;
-        std::vector<size_t> ctr(S, 0);
-        std::vector<uint8_t> mut(2 * (size_t)S);
-        while (ctr[S - 1] < ph[S - 1].size()) {
-            Score cost = 0.0;
-            std::fill(mut.begin(), mut.end(), 0);
-            for (uint32_t k = 0; k < n_trios; ++k) {
-                const uint32_t a = trios[3 * k], b = trios[3 * k + 1], c = trios[3 * k + 2];
-                const uint32_t sel_a = (t >> (2 * k)) & 1, sel_b = (t >> (2 * k + 1)) & 1;
-                const int child = ph[c][ctr[c]];
-                const int8_t ca = child & 1, cb = (child & 2) >> 1;
-                const int8_t pa = (ph[a][ctr[a]] & (1 + sel_a)) >> sel_a;
-                const int8_t pb = (ph[b][ctr[b]] & (1 + sel_b)) >> sel_b;
-                cost += (pa != ca) * mc[col];
-                cost += (pb != cb) * mc[col];
-                mut[2 * c] = (pa != ca);
-                mut[2 * c + 1] = (pb != cb);
-            }
-            for (uint32_t s = 0; s < S; ++s) cost += pc[(size_t)s * 5 + ph[s][ctr[s]]];
-            if (cost < best) {
-                best = cost;
-                if (alleles)
-                    for (uint32_t s = 0; s < S; ++s) {
-                        alleles[2 * s] = ph[s][ctr[s]] & 1;
-                        alleles[2 * s + 1] = (ph[s][ctr[s]] & 2) >> 1;
-                    }
-                if (mutated) std::copy(mut.begin(), mut.end(), mutated);
-            }
-            ++ctr[0];
-            for (uint32_t j = 0; j + 1 < S; ++j)
-                if (ctr[j] >= ph[j].size()) {
-                    ctr[j] = 0;
-                    ++ctr[j + 1];
-                }
-        }
-        return best;
     }
 
     // adds the votes of a read to one haplotype of its sample; returns the score the placement costs (addBalance, :562-585)
@@ -182,91 +107,12 @@ struct Solver {
 
 int Solver::run(whmec_heuristic_solution *out, std::string &err) {
     // ---- constructor part (:9-81)
-    n = p->n_cols;
-    m = p->n_reads;
-    n_trios = p->n_trios;
-    tm_bits = 2 * n_trios;
-    distrust = p->distrust != 0;
-    if (n > 0 && (!p->recombcost || !p->gt)) {
-        err = "recombcost and genotypes must be given for every column";
-        return WHMEC_ERR_INPUT;
-    }
-    if (m > 0 && (!p->read_off || !p->ent_col || !p->ent_allele || !p->ent_phred || !p->read_ind)) {
-        err = "read arrays must not be null";
-        return WHMEC_ERR_INPUT;
-    }
-    if (n_trios > 15) {
-        err = "unsupported pedigree: more than 15 trio relationships";
-        return WHMEC_ERR_UNSUPPORTED;
-    }
-    rc.assign(n, 0.0f);
-    mc.assign(n, std::numeric_limits<Score>::infinity());
-    for (uint32_t i = 1; i < n; ++i) {
-        rc[i] = (Score)p->recombcost[i];  // (rc[0] stays 0: recombinations are free in the first column)
-        if (allow_mut) mc[i - 1] = 0.75 * (rc[i - 1] + rc[i]);  // double product, stored as float
-    }
-    if (allow_mut && n > 0) mc[n - 1] = rc[n - 1] * 1.5;
-    // sample ids: those of the reads and of the trio members, ascending (Q3)
     {
-        std::vector<uint32_t> ids(p->read_ind, p->read_ind + m);
-        for (uint32_t i = 0; i < 3 * n_trios; ++i) ids.push_back(p->trios[i]);
-        std::sort(ids.begin(), ids.end());
-        ids.erase(std::unique(ids.begin(), ids.end()), ids.end());
-        S = (uint32_t)ids.size();
-        if (S > p->n_ind) {
-            err = "sample ids must be the zero-based indices of the pedigree's individuals";
-            return WHMEC_ERR_INPUT;
-        }
-        auto index_of = [&](uint32_t id) { return (uint32_t)(std::lower_bound(ids.begin(), ids.end(), id) - ids.begin()); };
-        sample_of_read.resize(m);
-        for (uint32_t r = 0; r < m; ++r) sample_of_read[r] = index_of(p->read_ind[r]);
-        trios.resize(3 * (size_t)n_trios);
-        for (uint32_t i = 0; i < 3 * n_trios; ++i) trios[i] = index_of(p->trios[i]);
-    }
-    out->n_samples = S;
-    out->score = 0;  // Q1
-    gt.assign((size_t)S * n, 0);
-    for (uint32_t s = 0; s < S; ++s)
-        for (uint32_t k = 0; k < n; ++k) {
-            const uint8_t g = p->gt[(size_t)s * n + k];
-            if (g > 2) {
-                err = "the heuristic needs a diploid biallelic genotype for every sample and column";
-                return WHMEC_ERR_INPUT;
-            }
-            gt[(size_t)s * n + k] = g;
-        }
-    first.resize(m);
-    last.resize(m);
-    for (uint32_t r = 0; r < m; ++r) {
-        const uint64_t b = p->read_off[r], e = p->read_off[r + 1];
-        if (e <= b) {
-            err = "No variants present";
-            return WHMEC_ERR_INPUT;
-        }
-        first[r] = p->ent_col[b];
-        last[r] = p->ent_col[e - 1];
-        if (last[r] >= n || first[r] > last[r] || (r > 0 && first[r] < first[r - 1])) {
-            err = "reads must be sorted by their first column and lie inside the columns";
-            return WHMEC_ERR_INPUT;
-        }
-    }
-    if (S == 0) {  // no reads and no trios: nothing to phase (the reference indexes an empty vector here)
-        if (out->transmission) std::fill(out->transmission, out->transmission + n, 0u);
-        return WHMEC_OK;
+        const int code = heur_prepare(*this, p, allow_mut, out, err);
+        if (code != WHMEC_OK || S == 0) return code;
     }
 
     // ---- solve (:121-409)
-    std::vector<uint32_t> start(1, 0);  // first read that starts after column k - 1
-    {
-        uint32_t q = 0;
-        for (uint32_t k = 0; k < n; ++k) {
-            while (q < m && first[q] <= k) ++q;
-            start.push_back(q);
-        }
-    }
-    std::vector<uint8_t> seen(S, 0);  // the first read of a sample that is not a child always goes to side 0
-    for (uint32_t k = 0; k < n_trios; ++k) seen[trios[3 * k + 2]] = 1;
-
     std::vector<Partial> prev(1);
     W = 1;
     prev[0].votes.assign(2 * (size_t)S, 0.0f);
@@ -482,8 +328,187 @@ int Solver::run(whmec_heuristic_solution *out, std::string &err) {
         tv[col] = tm_bits ? (tv_all[col][row] & (uint32_t)((1ull << tm_bits) - 1)) : 0u;
         row = back[col][row];
     }
-    if (out->partition) std::copy(part.begin(), part.end(), out->partition);
-    if (out->transmission) std::copy(tv.begin(), tv.end(), out->transmission);
+    heur_finish(*this, part.data(), tv.data(), out);
+    return WHMEC_OK;
+}
+
+}  // namespace
+
+namespace whmec {
+
+// best joint phasing of one column given the votes of all sample haplotypes (getOptPhasing, :462-560)
+HeurScore HeurTable::best_phasing(const std::vector<HeurScore> &v, uint32_t t, uint32_t col, int8_t *alleles, uint8_t *mutated) const {
+    using Score = HeurScore;
+    std::vector<Score> pc((size_t)S * 5);
+    for (uint32_t s = 0; s < S; ++s) {
+        const Score a0 = v[2 * s], a1 = v[2 * s + 1];
+        Score *c = &pc[(size_t)s * 5];
+        c[0] = (a0 * (a0 > 0) + a1 * (a1 > 0));
+        c[1] = (-a0 * (a0 < 0) + a1 * (a1 > 0));
+        c[2] = (a0 * (a0 > 0) - a1 * (a1 < 0));
+        c[3] = (-a0 * (a0 < 0) - a1 * (a1 < 0));
+        c[4] = *std::max_element(c, c + 4);
+    }
+    // allowed phasings per sample: 0 = 0|0, 1 = 0|1, 2 = 1|0, 3 = 1|1
+    std::vector<std::vector<int>> ph(S);
+    for (uint32_t s = 0; s < S; ++s) {
+        if (distrust) {
+            for (int i = 0; i < 4; ++i)
+                if (pc[(size_t)s * 5 + i] < pc[(size_t)s * 5 + 4] + 2 * mc[col]) ph[s].push_back(i);
+        } else {
+            const int g = gt[(size_t)s * n + col];
+            if (g == 0) ph[s].push_back(0);
+            else if (g == 2) ph[s].push_back(3);
+            else {
+                ph[s].push_back(1);
+                ph[s].push_back(2);
+            }
+        }
+    }
+    Score best = std::numeric_limits<Score>::infinity();
+    // (a sample without any allowed phasing -- possible with distrusted genotypes where the mutation cost is 0 -- makes the
+    //  reference index an empty vector, :505-530; here such a column has no finite phasing)
+    for (uint32_t s = 0; s < S; ++s)
+        if (ph[s].empty()) return best;
+    std::vector<size_t> ctr(S, 0);
+    std::vector<uint8_t> mut(2 * (size_t)S);
+    while (ctr[S - 1] < ph[S - 1].size()) {
+        Score cost = 0.0;
+        std::fill(mut.begin(), mut.end(), 0);
+        for (uint32_t k = 0; k < n_trios; ++k) {
+            const uint32_t a = trios[3 * k], b = trios[3 * k + 1], c = trios[3 * k + 2];
+            const uint32_t sel_a = (t >> (2 * k)) & 1, sel_b = (t >> (2 * k + 1)) & 1;
+            const int child = ph[c][ctr[c]];
+            const int8_t ca = child & 1, cb = (child & 2) >> 1;
+            const int8_t pa = (ph[a][ctr[a]] & (1 + sel_a)) >> sel_a;
+            const int8_t pb = (ph[b][ctr[b]] & (1 + sel_b)) >> sel_b;
+            cost += (pa != ca) * mc[col];
+            cost += (pb != cb) * mc[col];
+            mut[2 * c] = (pa != ca);
+            mut[2 * c + 1] = (pb != cb);
+        }
+        for (uint32_t s = 0; s < S; ++s) cost += pc[(size_t)s * 5 + ph[s][ctr[s]]];
+        if (cost < best) {
+            best = cost;
+            if (alleles)
+                for (uint32_t s = 0; s < S; ++s) {
+                    alleles[2 * s] = ph[s][ctr[s]] & 1;
+                    alleles[2 * s + 1] = (ph[s][ctr[s]] & 2) >> 1;
+                }
+            if (mutated) std::copy(mut.begin(), mut.end(), mutated);
+        }
+        ++ctr[0];
+        for (uint32_t j = 0; j + 1 < S; ++j)
+            if (ctr[j] >= ph[j].size()) {
+                ctr[j] = 0;
+                ++ctr[j + 1];
+            }
+    }
+    return best;
+}
+
+// constructor part (:9-81) and the start of solve (:121-140)
+int heur_prepare(HeurTable &tb, const whmec_problem *p, bool allow_mut, whmec_heuristic_solution *out, std::string &err) {
+    using Score = HeurScore;
+    tb.p = p;
+    tb.allow_mut = allow_mut;
+    uint32_t &n = tb.n, &m = tb.m, &S = tb.S, &n_trios = tb.n_trios;
+    std::vector<Score> &rc = tb.rc, &mc = tb.mc;
+    std::vector<uint32_t> &first = tb.first, &last = tb.last, &sample_of_read = tb.sample_of_read, &trios = tb.trios;
+    std::vector<int> &gt = tb.gt;
+    n = p->n_cols;
+    m = p->n_reads;
+    n_trios = p->n_trios;
+    tb.tm_bits = 2 * n_trios;
+    tb.distrust = p->distrust != 0;
+    if (n > 0 && (!p->recombcost || !p->gt)) {
+        err = "recombcost and genotypes must be given for every column";
+        return WHMEC_ERR_INPUT;
+    }
+    if (m > 0 && (!p->read_off || !p->ent_col || !p->ent_allele || !p->ent_phred || !p->read_ind)) {
+        err = "read arrays must not be null";
+        return WHMEC_ERR_INPUT;
+    }
+    if (n_trios > 15) {
+        err = "unsupported pedigree: more than 15 trio relationships";
+        return WHMEC_ERR_UNSUPPORTED;
+    }
+    rc.assign(n, 0.0f);
+    mc.assign(n, std::numeric_limits<Score>::infinity());
+    for (uint32_t i = 1; i < n; ++i) {
+        rc[i] = (Score)p->recombcost[i];  // (rc[0] stays 0: recombinations are free in the first column)
+        if (allow_mut) mc[i - 1] = 0.75 * (rc[i - 1] + rc[i]);  // double product, stored as float
+    }
+    if (allow_mut && n > 0) mc[n - 1] = rc[n - 1] * 1.5;
+    // sample ids: those of the reads and of the trio members, ascending (Q3)
+    {
+        std::vector<uint32_t> ids(p->read_ind, p->read_ind + m);
+        for (uint32_t i = 0; i < 3 * n_trios; ++i) ids.push_back(p->trios[i]);
+        std::sort(ids.begin(), ids.end());
+        ids.erase(std::unique(ids.begin(), ids.end()), ids.end());
+        S = (uint32_t)ids.size();
+        if (S > p->n_ind) {
+            err = "sample ids must be the zero-based indices of the pedigree's individuals";
+            return WHMEC_ERR_INPUT;
+        }
+        auto index_of = [&](uint32_t id) { return (uint32_t)(std::lower_bound(ids.begin(), ids.end(), id) - ids.begin()); };
+        sample_of_read.resize(m);
+        for (uint32_t r = 0; r < m; ++r) sample_of_read[r] = index_of(p->read_ind[r]);
+        trios.resize(3 * (size_t)n_trios);
+        for (uint32_t i = 0; i < 3 * n_trios; ++i) trios[i] = index_of(p->trios[i]);
+    }
+    out->n_samples = S;
+    out->score = 0;  // Q1
+    gt.assign((size_t)S * n, 0);
+    for (uint32_t s = 0; s < S; ++s)
+        for (uint32_t k = 0; k < n; ++k) {
+            const uint8_t g = p->gt[(size_t)s * n + k];
+            if (g > 2) {
+                err = "the heuristic needs a diploid biallelic genotype for every sample and column";
+                return WHMEC_ERR_INPUT;
+            }
+            gt[(size_t)s * n + k] = g;
+        }
+    first.resize(m);
+    last.resize(m);
+    for (uint32_t r = 0; r < m; ++r) {
+        const uint64_t b = p->read_off[r], e = p->read_off[r + 1];
+        if (e <= b) {
+            err = "No variants present";
+            return WHMEC_ERR_INPUT;
+        }
+        first[r] = p->ent_col[b];
+        last[r] = p->ent_col[e - 1];
+        if (last[r] >= n || first[r] > last[r] || (r > 0 && first[r] < first[r - 1])) {
+            err = "reads must be sorted by their first column and lie inside the columns";
+            return WHMEC_ERR_INPUT;
+        }
+    }
+    if (S == 0) {  // no reads and no trios: nothing to phase (the reference indexes an empty vector here)
+        if (out->transmission) std::fill(out->transmission, out->transmission + n, 0u);
+        return WHMEC_OK;
+    }
+    std::vector<uint32_t> &start = tb.start;
+    start.assign(1, 0);  // first read that starts after column k - 1
+    {
+        uint32_t q = 0;
+        for (uint32_t k = 0; k < n; ++k) {
+            while (q < m && first[q] <= k) ++q;
+            start.push_back(q);
+        }
+    }
+    tb.seen.assign(S, 0);  // the first read of a sample that is not a child always goes to side 0
+    for (uint32_t k = 0; k < n_trios; ++k) tb.seen[trios[3 * k + 2]] = 1;
+    return WHMEC_OK;
+}
+
+void heur_finish(const HeurTable &tb, const uint8_t *part, const uint32_t *tv, whmec_heuristic_solution *out) {
+    using Score = HeurScore;
+    const whmec_problem *p = tb.p;
+    const uint32_t n = tb.n, m = tb.m, S = tb.S;
+    const std::vector<uint32_t> &sample_of_read = tb.sample_of_read;
+    if (out->partition) std::copy(part, part + m, out->partition);
+    if (out->transmission) std::copy(tv, tv + n, out->transmission);
 
     // votes of all reads under the chosen bipartition, then the best phasing of every column
     std::vector<Score> votes((size_t)n * 2 * S, 0.0f);
@@ -493,7 +518,6 @@ int Solver::run(whmec_heuristic_solution *out, std::string &err) {
             const Score q = (Score)(int)p->ent_phred[e];
             if (a >= 0) votes[(size_t)p->ent_col[e] * 2 * S + 2 * sample_of_read[r] + part[r]] += (2 * a - 1) * q;
         }
-    W = 1;
     std::vector<int8_t> alleles(2 * (size_t)S);
     std::vector<uint8_t> mutated(2 * (size_t)S);
     if (out->mutated) std::memset(out->mutated, 0, (size_t)S * 2 * n);
@@ -501,17 +525,16 @@ int Solver::run(whmec_heuristic_solution *out, std::string &err) {
         std::vector<Score> v(votes.begin() + (size_t)col * 2 * S, votes.begin() + (size_t)(col + 1) * 2 * S);
         std::fill(alleles.begin(), alleles.end(), 0);
         std::fill(mutated.begin(), mutated.end(), 0);
-        best_phasing(v, tv[col], col, alleles.data(), mutated.data());
+        tb.best_phasing(v, tv[col], col, alleles.data(), mutated.data());
         for (uint32_t s = 0; s < S; ++s)
             for (uint32_t h = 0; h < 2; ++h) {
                 if (out->haplotypes) out->haplotypes[((size_t)s * 2 + h) * n + col] = alleles[2 * s + h];
                 if (out->mutated) out->mutated[((size_t)s * 2 + h) * n + col] = mutated[2 * s + h];
             }
     }
-    return WHMEC_OK;
 }
 
-}  // namespace
+}  // namespace whmec
 
 extern "C" int whmec_heuristic(const whmec_problem *p, uint32_t row_limit, int allow_mutations, whmec_heuristic_solution *s, char *err,
                                size_t errlen) {
@@ -519,8 +542,8 @@ extern "C" int whmec_heuristic(const whmec_problem *p, uint32_t row_limit, int a
     int rc;
     try {
         Solver sv;
-        sv.p = p;
         sv.row_limit = std::min(row_limit, MAX_ROWS);
+        sv.p = p;
         sv.allow_mut = allow_mutations != 0;
         rc = sv.run(s, msg);
     } catch (const std::bad_alloc &) {

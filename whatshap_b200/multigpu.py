@@ -887,6 +887,54 @@ def genotype_tables(problems: Sequence[FlatProblem], device: int = 0, devices: O
                    lambda p: float(block_work(p, [(0, p.n_cols)])[0]) * 4.0 ** p.n_trios * 2.0 ** (2 * (p.n_ind - p.n_trios)))
 
 
+def heuristic_tables(problems: Sequence[FlatProblem], row_limits=256, allow_mutations=True, device: int = 0,
+                     devices: Optional[Sequence[int]] = None, with_stats: bool = False):
+    """Several heuristic tables at once: per table, in input order, its `HeuristicSolution` or the exception `_lib.heuristic` would
+    have raised for it (a failure of the device raises, whatever the length of the list).  `row_limits` / `allow_mutations`: per
+    table, or one value for all.  On one device this is `_lib.heuristic_batch` (one CTA per table).  With `devices` /
+    WHMEC_DEVICES whole tables go to devices by longest-processing-time-first on columns x row_limit (`assign_blocks`), one
+    `whmec_heuristic_batch` per device on that device's host thread; a single table runs on the first device.  `with_stats`:
+    (results, per-table stats) instead."""
+    from . import _lib
+
+    problems = list(problems)
+    n = len(problems)
+    limits = [int(row_limits)] * n if isinstance(row_limits, (int, np.integer)) else [int(r) for r in row_limits]
+    allow = [bool(allow_mutations)] * n if isinstance(allow_mutations, (bool, int, np.integer)) else [bool(a) for a in allow_mutations]
+    if len(limits) != n or len(allow) != n:
+        raise ValueError("row_limits and allow_mutations need one entry per table")
+
+    # the driver sees table positions, so that every table keeps its own row limit and flag
+    def batch(ids, d):
+        return _lib.heuristic_batch([problems[i] for i in ids], [limits[i] for i in ids], [allow[i] for i in ids], device=d, with_stats=True)
+
+    def single(i, dev, devs):
+        chosen = table_devices(dev, devs)
+        res, (st, _) = batch([i], chosen[0] if chosen else dev)
+        if isinstance(res[0], BaseException):
+            raise res[0]
+        return res[0], st[0]
+
+    return _tables(list(range(n)), device, devices, with_stats, batch, single,
+                   lambda i: float(problems[i].n_cols) * max(1, min(limits[i], 65535)))
+
+
+def batch_heuristic_objects(cls, tables, setup, device: int, devices: Optional[Sequence[int]], return_exceptions: bool) -> list:
+    """The `batch` classmethods of the PedMecHeuristic classes: `setup(obj, args)` does the constructor's work up to the solver
+    for one argument tuple `(readset, recombcost, pedigree[, row_limit[, distrust_genotypes[, positions[, allow_mutations[,
+    verbosity]]]]])`, then every table's row limit (capped to 0..65535, as the constructor does) and flag go with its problem
+    to `heuristic_tables`.  Errors as in `batch_objects`."""
+    options: list = []
+
+    def build(obj, args):
+        setup(obj, args)
+        row_limit = min(max(int(args[3]), 0), 65535) if len(args) > 3 else 256
+        options.append((row_limit, bool(args[6]) if len(args) > 6 else True))
+
+    return batch_objects(cls, tables, build, lambda problems: heuristic_tables(problems, [o[0] for o in options], [o[1] for o in options], device,
+                                                                               devices, with_stats=True), "_solution", return_exceptions)
+
+
 def batch_objects(cls, tables, build, run, attr: str, return_exceptions: bool) -> list:
     """The `batch` classmethods of the table classes: one `cls` object per constructor argument tuple of `tables`
     (`build(obj, args)` fills it; an exception it raises takes the table's place), `run(problems)` -> (results, per-table stats or
