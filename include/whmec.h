@@ -18,6 +18,8 @@
  *   whmec_genotype         <- GenotypeDPTable::GenotypeDPTable  src/genotypedptable.cpp:17-48 (ctor runs the
  *                             backward and the forward pass :118-215) + get_genotype_likelihoods :445-451,
  *                             bound at whatshap/core.pyx:581-600  (sibling DP, SURVEY.md 8(f) rank 4)
+ *   whmec_realign          <- ReadSetReader.detect_alleles_by_alignment  whatshap/variants.py:599-912 (allele detection
+ *                             by re-alignment, the step that builds the ReadSet)
  *
  * Plain pointers and sizes only.  All input pointers are caller-owned host
  * memory, read-only, and need to stay valid only for the duration of the call.
@@ -329,6 +331,67 @@ int whmec_heuristic_batch(const whmec_problem *const *problems, whmec_heuristic_
                           const int *allow_mutations /* [n_tables] */, uint32_t n_tables, int device, int *status /* [n_tables] */,
                           char *errs /* [n_tables][errlen] or NULL */, size_t errlen, whmec_stats *stats_or_null /* [n_tables] */,
                           whmec_stats *total_or_null);
+
+/* ---- Allele detection by re-alignment: ReadSetReader.detect_alleles_by_alignment(variants, restricted_genotypes, 0, alignment,
+ * reference, overhang, use_affine, gap_start, gap_extend, default_mismatch) for many alignments in one call
+ * (whatshap/variants.py:599-912, whatshap/_variants.pyx:10-81, whatshap/align.pyx:16-196).  kmer alignment is not covered.
+ * The host walks every CIGAR against the variant list (WHMEC_HOST_THREADS workers) and lists the (alignment, variant) items and
+ * their alleles; the device builds each padded allele from the reference, strips common prefix and suffix, computes every
+ * allele's distance and makes the call.  Work goes in chunks of items under the free HBM (or WHMEC_REALIGN_ARENA_BUDGET bytes). */
+typedef struct whmec_realign_input {
+    uint32_t n_alignments;
+    const int32_t *reference_start;  /* [n_alignments] */
+    const uint64_t *cigar_off;       /* [n_alignments + 1] into cigar_op / cigar_len; an empty CIGAR yields nothing */
+    const uint8_t *cigar_op;         /* pysam codes MIDNSHP=X = 0..8; others raise when the walk reaches them */
+    const int32_t *cigar_len;
+    const uint64_t *query_off;       /* [n_alignments + 1] into query */
+    const uint8_t *query;            /* query_sequence bytes, compared case-sensitively */
+    uint32_t n_variants;
+    const int32_t *position;         /* [n_variants] */
+    const uint32_t *allele_first;    /* [n_variants + 1]: variant v's alleles are slots allele_first[v] .. allele_first[v+1]-1, reference allele first */
+    const uint64_t *allele_off;      /* [allele_first[n_variants] + 1] into allele_bytes */
+    const uint8_t *allele_bytes;
+    const uint64_t *restrict_off;    /* NULL: no restricted genotypes; else [n_variants + 1] into restrict_allele */
+    const int32_t *restrict_allele;  /* per variant: the allele indices of its genotype (Genotype.as_vector()) */
+    const uint8_t *reference;
+    uint64_t reference_len;
+    int32_t overhang;                /* >= 0 */
+    int32_t affine;                  /* 0: edit_distance (quality 30); 1: edit_distance_affine_gap (quality d_best - d_second) */
+    int32_t gap_start, gap_extend;
+    double mismatch;                 /* default_mismatch, used as a float32 */
+} whmec_realign_input;
+
+typedef struct whmec_realign_output { /* filled by the library; release with whmec_realign_release */
+    uint64_t *call_off;              /* [n_alignments + 1] into the three arrays below */
+    uint32_t *variant;               /* index into the variant list */
+    int32_t *allele;
+    int64_t *quality;
+} whmec_realign_output;
+
+typedef struct whmec_realign_stats {
+    uint64_t items;                  /* (alignment, variant) pairs aligned */
+    uint64_t jobs;                   /* allele alignments */
+    uint64_t short_jobs, long_jobs;  /* one thread per job / one warp per job */
+    uint64_t long_items;             /* items with at least one warp job */
+    uint64_t cells;                  /* sum of untrimmed query x target lengths */
+    uint64_t h2d_bytes, d2h_bytes;
+    uint32_t chunks, kernel_launches;
+    float device_ms;                 /* device time of the launches (CUDA events) */
+    float plan_ms;                   /* host walk */
+} whmec_realign_stats;
+
+/* Returns WHMEC_OK, WHMEC_ERR_INPUT for malformed arguments and for every input on which the reference raises (an unknown CIGAR
+ * operation, a failed window assert, an empty allele list after the restriction, a distance beyond int64): err then names the
+ * first such alignment (and variant); WHMEC_ERR_CUDA for a device failure.  out is only filled on WHMEC_OK.  stats may be NULL. */
+int whmec_realign(const whmec_realign_input *in, int device, whmec_realign_output *out, whmec_realign_stats *stats, char *err,
+                  size_t errlen);
+void whmec_realign_release(whmec_realign_output *out);
+
+/* edit_distance(query[i], target[i]) and edit_distance_affine_gap(query[i], target[i], [mismatch] * len(query[i]), gap_start,
+ * gap_extend) for n pairs (align.pyx:16-196); either output may be NULL.  Return codes as whmec_realign. */
+int whmec_edit_distance_batch(uint32_t n, const uint64_t *query_off, const uint8_t *query, const uint64_t *target_off,
+                              const uint8_t *target, double mismatch, int32_t gap_start, int32_t gap_extend, int64_t *unit_out,
+                              int64_t *affine_out, int device, whmec_realign_stats *stats, char *err, size_t errlen);
 
 #ifdef __cplusplus
 }

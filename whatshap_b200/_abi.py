@@ -298,3 +298,60 @@ def raise_for(rc: int, msg: str):
     if rc == WHMEC_ERR_UNSUPPORTED:
         raise Unsupported(f"unsupported problem: {msg}")
     raise RuntimeError(f"whmec error {rc}: {msg}")
+
+
+class CRealignInput(C.Structure):
+    """whmec_realign_input: alignments, variants, restricted genotypes, reference and costs of one whmec_realign call."""
+    _fields_ = [
+        ("n_alignments", C.c_uint32),
+        ("reference_start", C.POINTER(C.c_int32)),
+        ("cigar_off", _u64p),
+        ("cigar_op", _u8p),
+        ("cigar_len", C.POINTER(C.c_int32)),
+        ("query_off", _u64p),
+        ("query", _u8p),
+        ("n_variants", C.c_uint32),
+        ("position", C.POINTER(C.c_int32)),
+        ("allele_first", _u32p),
+        ("allele_off", _u64p),
+        ("allele_bytes", _u8p),
+        ("restrict_off", _u64p),
+        ("restrict_allele", C.POINTER(C.c_int32)),
+        ("reference", _u8p),
+        ("reference_len", C.c_uint64),
+        ("overhang", C.c_int32),
+        ("affine", C.c_int32),
+        ("gap_start", C.c_int32),
+        ("gap_extend", C.c_int32),
+        ("mismatch", C.c_double),
+    ]
+
+
+class CRealignOutput(C.Structure):
+    """whmec_realign_output: per alignment (CSR) the calls (variant index, allele, quality); the library owns the arrays."""
+    _fields_ = [
+        ("call_off", _u64p),
+        ("variant", _u32p),
+        ("allele", C.POINTER(C.c_int32)),
+        ("quality", C.POINTER(C.c_int64)),
+    ]
+
+
+class CRealignStats(C.Structure):
+    _fields_ = [
+        ("items", C.c_uint64),
+        ("jobs", C.c_uint64),
+        ("short_jobs", C.c_uint64),
+        ("long_jobs", C.c_uint64),
+        ("long_items", C.c_uint64),
+        ("cells", C.c_uint64),
+        ("h2d_bytes", C.c_uint64),
+        ("d2h_bytes", C.c_uint64),
+        ("chunks", C.c_uint32),
+        ("kernel_launches", C.c_uint32),
+        ("device_ms", C.c_float),
+        ("plan_ms", C.c_float),
+    ]
+
+    def as_dict(self) -> dict:
+        return {name: getattr(self, name) for name, _ in self._fields_}

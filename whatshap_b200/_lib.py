@@ -13,7 +13,7 @@ from typing import List, Optional, Sequence, Tuple, Union
 
 import numpy as np
 
-from ._abi import CHeuristicSolution, CProblem, CSolution, CStats, FlatProblem, FlatSolution, HeuristicSolution, raise_for
+from ._abi import CHeuristicSolution, CProblem, CRealignInput, CRealignOutput, CRealignStats, CSolution, CStats, FlatProblem, FlatSolution, HeuristicSolution, raise_for
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("WHMEC_LIBRARY") or os.path.join(HERE, "libwhmec.so")  # WHMEC_LIBRARY: another build of the same library (A/B runs)
@@ -51,6 +51,9 @@ EXPORTS = (
     "whmec_compute_genotypes",
     "whmec_heuristic",
     "whmec_heuristic_batch",
+    "whmec_realign",
+    "whmec_realign_release",
+    "whmec_edit_distance_batch",
 )
 
 
@@ -124,12 +127,27 @@ def lib() -> C.CDLL:
     L.whmec_genotype_segment_run.argtypes = [C.c_void_p, f64p, f64p, f64p, C.POINTER(CStats), C.c_char_p, C.c_size_t]
     L.whmec_genotype_segment_destroy.argtypes = [C.c_void_p]
     L.whmec_genotype_segment_destroy.restype = None
+    realign_signatures(L)
     for name in ("whmec_genotype_segment_create", "whmec_genotype_segment_transfer", "whmec_genotype_segment_run"):
         getattr(L, name).restype = C.c_int
     for name in ("whmec_plan_create", "whmec_plan_sweep", "whmec_plan_finish", "whmec_plan_stats", "whmec_solve",
                  "whmec_segment_create", "whmec_segment_transfer", "whmec_segment_sweep", "whmec_segment_exits",
                  "whmec_segment_finish"):
         getattr(L, name).restype = C.c_int
+    return L
+
+
+def realign_signatures(L: C.CDLL) -> C.CDLL:
+    """argtypes of whmec_realign, whmec_realign_release and whmec_edit_distance_batch on `L` (this library or a test build that
+    exports the same three symbols)."""
+    i64p = C.POINTER(C.c_int64)
+    L.whmec_realign.argtypes = [C.POINTER(CRealignInput), C.c_int, C.POINTER(CRealignOutput), C.POINTER(CRealignStats), C.c_char_p, C.c_size_t]
+    L.whmec_realign.restype = C.c_int
+    L.whmec_realign_release.argtypes = [C.POINTER(CRealignOutput)]
+    L.whmec_realign_release.restype = None
+    L.whmec_edit_distance_batch.argtypes = [C.c_uint32, C.POINTER(C.c_uint64), C.POINTER(C.c_uint8), C.POINTER(C.c_uint64), C.POINTER(C.c_uint8),
+                                            C.c_double, C.c_int32, C.c_int32, i64p, i64p, C.c_int, C.POINTER(CRealignStats), C.c_char_p, C.c_size_t]
+    L.whmec_edit_distance_batch.restype = C.c_int
     return L
 
 

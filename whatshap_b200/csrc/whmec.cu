@@ -2563,3 +2563,8 @@ int whmec_solve_batch(const whmec_problem *const *problems, whmec_solution *cons
 }
 
 }  // extern "C"
+
+namespace whmec {
+// The page-locked staging pool behind StagedVec, for entry points whose device code lives in other files (realign.cu).
+void install_pinned_staging() { install_stage_hooks(); }
+}  // namespace whmec

@@ -1,0 +1,174 @@
+"""Allele detection by re-alignment on the GPU, for many alignments in one call.
+
+`detect_alleles` gives, per alignment, the list of (variant index, allele, quality) that WhatsHap's
+`ReadSetReader.detect_alleles_by_alignment(variants, restricted_genotypes, 0, alignment, reference, overhang, use_affine,
+gap_start, gap_extend, default_mismatch)` yields, in the same order (whatshap/variants.py:599-912): the host walks every CIGAR
+against the variant list, the device aligns each covered variant's query window against its padded alleles
+(`whmec_realign`, DESIGN §4.11).  `edit_distances` and `edit_distances_affine_gap` are `whatshap.align.edit_distance` and
+`edit_distance_affine_gap` (with one mismatch cost for every query position) over many pairs.
+
+Where the reference raises (an unknown CIGAR operation, a failed window assert, a restricted genotype that leaves no allele),
+the call raises ValueError naming the first such alignment and variant.  Inputs the reference would only reject later are
+rejected up front: affine mode without its three costs, a negative overhang, a CIGAR without a query sequence, fewer
+restricted genotypes than variants.  kmer alignment (`--use-kmerald`) is not covered.
+"""
+from __future__ import annotations
+
+import ctypes as C
+from typing import List, Optional, Sequence, Tuple
+
+import numpy as np
+
+from . import _lib
+from ._abi import WHMEC_ERR_INPUT, CRealignInput, CRealignOutput, CRealignStats, raise_for
+
+Call = Tuple[int, int, int]
+
+
+def _bytes(s) -> bytes:
+    return s.encode() if isinstance(s, str) else bytes(s)
+
+
+def _ptr(a: Optional[np.ndarray], ctype):
+    return C.cast(None, C.POINTER(ctype)) if a is None else a.ctypes.data_as(C.POINTER(ctype))
+
+
+def _csr(chunks: Sequence[bytes]) -> Tuple[np.ndarray, np.ndarray]:
+    off = np.zeros(len(chunks) + 1, np.uint64)
+    if chunks:
+        np.cumsum(np.fromiter(map(len, chunks), np.uint64, len(chunks)), out=off[1:])
+    buf = np.frombuffer(b"".join(chunks), np.uint8) if off[-1] else np.zeros(1, np.uint8)
+    return off, buf
+
+
+def _int32(values, what: str) -> np.ndarray:
+    a = np.asarray(values, dtype=np.int64)
+    if a.size and (a.min() < -(2**31) or a.max() >= 2**31):
+        raise ValueError(f"{what} outside the 32-bit range of the reference's C ints")
+    return a.astype(np.int32)
+
+
+def pack_input(alignments, variants, reference, restricted_genotypes=None, overhang=10, affine=False, gap_start=None,
+               gap_extend=None, default_mismatch=None):
+    """(whmec_realign_input, the arrays it points into): the flat form of one detect_alleles call."""
+    if overhang < 0:
+        raise ValueError("overhang must be >= 0")
+    if affine and (gap_start is None or gap_extend is None or default_mismatch is None):
+        raise ValueError("affine realignment needs gap_start, gap_extend and default_mismatch")
+    keep = []
+    n = len(alignments)
+    cigars = [a.cigartuples or () for a in alignments]
+    queries = []
+    for k, (a, cg) in enumerate(zip(alignments, cigars)):
+        seq = a.query_sequence
+        if seq is None and cg:
+            raise ValueError(f"alignment {k} has a CIGAR but no query sequence")
+        queries.append(_bytes(seq) if seq is not None else b"")
+    starts = _int32([a.reference_start for a in alignments], "reference_start")
+    cigar_off = np.zeros(n + 1, np.uint64)
+    if n:
+        np.cumsum(np.fromiter(map(len, cigars), np.uint64, n), out=cigar_off[1:])
+    flat = np.array([x for cg in cigars for x in cg], dtype=np.int64).reshape(-1, 2)
+    ops = flat[:, 0]
+    cigar_op = np.where((ops >= 0) & (ops <= 254), ops, 255).astype(np.uint8)
+    cigar_len = _int32(flat[:, 1], "CIGAR length")
+    query_off, query = _csr(queries)
+    positions = _int32([v.position for v in variants], "variant position")
+    alleles, first = [], [0]
+    for v in variants:
+        alleles.append(_bytes(v.reference_allele))
+        alleles.extend(_bytes(x) for x in v.get_alt_allele_list())
+        first.append(len(alleles))
+    allele_first = np.array(first, np.uint32)
+    allele_off, allele_bytes = _csr(alleles)
+    r_off = r_all = None
+    if restricted_genotypes:
+        if len(restricted_genotypes) < len(variants):
+            raise ValueError("restricted_genotypes has fewer entries than variants")
+        vecs = [list(restricted_genotypes[i].as_vector()) for i in range(len(variants))]
+        r_off = np.zeros(len(vecs) + 1, np.uint64)
+        if vecs:
+            np.cumsum(np.fromiter(map(len, vecs), np.uint64, len(vecs)), out=r_off[1:])
+        r_all = np.clip(np.array([x for g in vecs for x in g] or [0], np.int64), -1, 2**31 - 1).astype(np.int32)
+    ref = np.frombuffer(_bytes(reference), np.uint8) if len(reference) else np.zeros(1, np.uint8)
+    keep += [starts, cigar_off, cigar_op, cigar_len, query_off, query, positions, allele_first, allele_off, allele_bytes, r_off, r_all, ref]
+    ci = CRealignInput(
+        n, _ptr(starts, C.c_int32), _ptr(cigar_off, C.c_uint64), _ptr(cigar_op, C.c_uint8), _ptr(cigar_len, C.c_int32),
+        _ptr(query_off, C.c_uint64), _ptr(query, C.c_uint8), len(variants), _ptr(positions, C.c_int32), _ptr(allele_first, C.c_uint32),
+        _ptr(allele_off, C.c_uint64), _ptr(allele_bytes, C.c_uint8), _ptr(r_off, C.c_uint64), _ptr(r_all, C.c_int32),
+        _ptr(ref, C.c_uint8), len(reference), int(overhang), int(bool(affine)),
+        int(gap_start) if affine else 0, int(gap_extend) if affine else 0, float(default_mismatch) if affine else 0.0)
+    return ci, keep
+
+
+def detect_alleles(alignments, variants, reference, *, restricted_genotypes=None, overhang: int = 10, affine: bool = False,
+                   gap_start=None, gap_extend=None, default_mismatch=None, device: int = 0, stats: Optional[dict] = None,
+                   library: Optional[C.CDLL] = None) -> List[List[Call]]:
+    """Per alignment, the (variant index, allele, quality) tuples of detect_alleles_by_alignment, in its order.
+
+    alignments: objects with `reference_start`, `cigartuples` and `query_sequence` (a pysam.AlignedSegment qualifies);
+    variants: objects with `position`, `reference_allele` and `get_alt_allele_list()`; reference: the chromosome (str or
+    bytes); restricted_genotypes: None or one object with `as_vector()` per variant.  `stats` (a dict) receives the
+    call's counters: items, jobs, short_jobs / long_jobs (one thread / one warp per allele alignment), chunks, device_ms.
+    `library`: another build of the library with the same entry point (tests)."""
+    L = library or _lib.lib()
+    ci, keep = pack_input(alignments, variants, reference, restricted_genotypes, overhang, affine, gap_start, gap_extend, default_mismatch)
+    out, st = CRealignOutput(), CRealignStats()
+    err = C.create_string_buffer(1024)
+    rc = L.whmec_realign(C.byref(ci), device, C.byref(out), C.byref(st), err, len(err))
+    if rc == WHMEC_ERR_INPUT:
+        raise ValueError(err.value.decode())
+    raise_for(rc, err.value.decode())
+    try:
+        n = len(alignments)
+        off = np.ctypeslib.as_array(out.call_off, (n + 1,)).copy()
+        total = int(off[-1])
+        if total:
+            var = np.ctypeslib.as_array(out.variant, (total,)).tolist()
+            al = np.ctypeslib.as_array(out.allele, (total,)).tolist()
+            ql = np.ctypeslib.as_array(out.quality, (total,)).tolist()
+        else:
+            var = al = ql = []
+    finally:
+        L.whmec_realign_release(C.byref(out))
+    del keep
+    if stats is not None:
+        stats.update(st.as_dict())
+    calls = list(zip(var, al, ql))
+    return [calls[off[k]:off[k + 1]] for k in range(n)]
+
+
+def _pairs(queries, targets, mismatch, gap_start, gap_extend, affine, device, stats, library):
+    if len(queries) != len(targets):
+        raise ValueError("queries and targets differ in length")
+    L = library or _lib.lib()
+    n = len(queries)
+    q_off, q = _csr([_bytes(s) for s in queries])
+    t_off, t = _csr([_bytes(s) for s in targets])
+    res = np.zeros(max(n, 1), np.int64)
+    st = CRealignStats()
+    err = C.create_string_buffer(512)
+    i64 = C.POINTER(C.c_int64)
+    dst = res.ctypes.data_as(i64)
+    none = C.cast(None, i64)
+    rc = L.whmec_edit_distance_batch(n, _ptr(q_off, C.c_uint64), _ptr(q, C.c_uint8), _ptr(t_off, C.c_uint64), _ptr(t, C.c_uint8),
+                                     float(mismatch), int(gap_start), int(gap_extend), none if affine else dst, dst if affine else none,
+                                     device, C.byref(st), err, len(err))
+    if rc == WHMEC_ERR_INPUT:
+        raise ValueError(err.value.decode())
+    raise_for(rc, err.value.decode())
+    if stats is not None:
+        stats.update(st.as_dict())
+    return res[:n]
+
+
+def edit_distances(queries, targets, *, device: int = 0, stats: Optional[dict] = None, library: Optional[C.CDLL] = None) -> np.ndarray:
+    """edit_distance(queries[i], targets[i]) (unit costs, align.pyx:16-109) for every i, as int64."""
+    return _pairs(queries, targets, 0.0, 0, 0, False, device, stats, library)
+
+
+def edit_distances_affine_gap(queries, targets, mismatch, gap_start: int = 1, gap_extend: int = 1, *, device: int = 0,
+                              stats: Optional[dict] = None, library: Optional[C.CDLL] = None) -> np.ndarray:
+    """int(edit_distance_affine_gap(queries[i], targets[i], [mismatch] * len(queries[i]), gap_start, gap_extend)) for every i
+    (align.pyx:114-196): the float32 Gotoh recurrence, mismatch as a float32, gap costs as C ints (10.9 -> 10)."""
+    return _pairs(queries, targets, mismatch, int(gap_start), int(gap_extend), True, device, stats, library)
