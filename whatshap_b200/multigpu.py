@@ -2,30 +2,33 @@
 
 For a single individual (T = 1) the DP decomposes exactly at columns that no read spans: cost adds,
 partitioning / super-reads concatenate, tie-breaks are unaffected (a constant offset changes no `<`).
-Those blocks are the unit of work: rank 0 scatters to every rank (one process per GPU,
-`torch.distributed` over NCCL) the blocks of its share, each rank solves them through the C ABI with
-no collective on the data path, and the per-block results are gathered on rank 0.  Pedigrees (T > 1)
-couple the blocks through the transmission vector: every rank holds a SEGMENT of the table
-(`whmec_segment_*`) and the ranks exchange T x T transfer matrices and exit tables (two all-gathers of a
-few hundred bytes), bit-identical to the single-GPU solve.  `genotype_sharded` does the same by chains for the
-forward-backward genotyping DP of a single individual, and by segments of the table for a pedigree: every rank holds a
-segment (`whmec_genotype_segment_*`), the ranks all-gather T x T transfer matrices of doubles, fold them into every
-segment's true forward and backward inputs, and each runs its segment (DESIGN §4.5).
+Runs of those blocks are the parts of the table (`plan_parts`), solved with no exchange between them and merged in column
+order.  Pedigrees (T > 1) couple the blocks through the transmission vector: every part is a SEGMENT of the table
+(`whmec_segment_*`) and the parts exchange T x T transfer matrices and exit tables, bit-identical to the single-GPU solve.
+Genotyping (the forward-backward DP) cuts a single individual by chains and a pedigree into segments
+(`whmec_genotype_segment_*`) that exchange T x T transfer matrices of doubles, folded into every segment's true forward and
+backward inputs (DESIGN §4.5).
 
-`solve_on_devices` / `genotype_on_devices` make the same cuts in ONE process (no process group): one host thread per
-device, the folds on the calling thread.  `core`'s tables and the swap-in classes of `adapters` reach them through
-`solve_table` / `genotype_table` when given `devices` or when WHMEC_DEVICES is set (DESIGN §6).
+Each scheme is written once (`_phasing_segments`, `_genotype_segments`, and `_run_parts` for runs of blocks and for the
+whole table) and runs on one of three executors: `_Local` (every part in one process on one device, in column order:
+`solve_pedigree_segments`, `genotype_pedigree_segments`), `_Threads` (one host thread per device in one process:
+`solve_on_devices`, `genotype_on_devices`, which `core`'s tables and the swap-in classes of `adapters` reach through
+`solve_table` / `genotype_table` when given `devices` or when WHMEC_DEVICES is set) and `_Ranks` (one process per GPU,
+`torch.distributed` over NCCL: `solve_sharded`, `genotype_sharded`).  DESIGN §6.
 
 The reference has no counterpart (single process, `whatshap/cli/phase.py:604-610` runs one
 PedigreeDPTable per chromosome x family).
 """
 from __future__ import annotations
 
+import os
+import time
 from typing import Callable, List, Optional, Sequence, Tuple
 
 import numpy as np
 
-from ._abi import FlatProblem, FlatSolution
+from . import _wire
+from ._abi import FlatProblem, FlatSolution, Unsupported
 
 
 def _read_spans(prob: FlatProblem) -> Tuple[np.ndarray, np.ndarray]:
@@ -182,15 +185,6 @@ def segment_entries(exits: Sequence[Optional[np.ndarray]]) -> List[Optional[int]
     return entries
 
 
-def _default_segment_factory():
-    import torch
-
-    from . import _lib
-
-    device = torch.cuda.current_device()
-    return lambda p, continues: _lib.Segment(p, continues, device=device)
-
-
 def segment_ranges(prob: FlatProblem, world: int) -> List[Optional[Tuple[int, int]]]:
     """Column range [lo, hi) of every rank's segment (None: no columns for that rank)."""
     blocks = independent_blocks(prob)
@@ -214,194 +208,6 @@ def plan_parts(prob: FlatProblem, world: int, genotype: bool = False, spans=None
         return ("segments", segment_ranges(prob, world)) if world > 1 and len(blocks) > 1 else ("whole", [])
     runs = contiguous_shares(block_work(prob, blocks, spans), world)
     return "blocks", [(blocks[b0][0], blocks[b1 - 1][1]) if b1 > b0 else None for b0, b1 in runs]
-
-
-def solve_pedigree_segments(prob: FlatProblem, n_segments: int, segment_factory=None) -> FlatSolution:
-    """The multi-GPU pedigree scheme with all `n_segments` segments driven by ONE process on one
-    device, in the order the ranks would run them -- the single-GPU check of `whmec_segment_*`
-    (tests/test_gpu_sharded.py) and of this module's folding logic."""
-    if segment_factory is None:
-        segment_factory = _default_segment_factory()
-    ranges = segment_ranges(prob, n_segments)
-    segs = [None if r is None else segment_factory(prob.slice_columns(*r), r[0] > 0) for r in ranges]
-    try:
-        last_active = max(i for i, sg in enumerate(segs) if sg is not None)
-        inputs = segment_inputs([sg.transfer() if sg else None for sg in segs])
-        for sg, vec in zip(segs, inputs):
-            if sg:
-                sg.sweep(vec)
-        entries = segment_entries([sg.exits(i == last_active) if sg else None for i, sg in enumerate(segs)])
-        parts = [(ranges[i], sg.finish(entries[i])) for i, sg in enumerate(segs) if sg]
-    finally:
-        for sg in segs:
-            if sg:
-                sg.close()
-    return merge_block_solutions(prob, [r for r, _ in parts], [sol for _, sol in parts], cost=int(parts[-1][1].cost))
-
-
-def solve_pedigree_sharded(prob: Optional[FlatProblem], segment_factory=None, group=None, ranges=None,
-                           my_slice: Optional[FlatProblem] = None, comm=None, timings: Optional[dict] = None
-                           ) -> Tuple[bool, Optional[FlatSolution]]:
-    """T > 1.  Every rank holds its segment of the table: either `prob` is known on every rank (each slices its own
-    range), or `ranges` (all ranks' column ranges) and `my_slice` (this rank's columns, None for a rank without columns)
-    are given and only rank 0 needs `prob` (for merging).  Returns (True, solution) on rank 0 and (True, None)
-    elsewhere, or (False, None) on every rank if some segment is outside what the two-pass scheme handles (the
-    caller then solves on one GPU).  Every rank-local phase reports its status in the all-gather that follows it, so an
-    error on one rank (Mendelian conflict, unsorted reads, a CUDA failure) is raised on EVERY rank."""
-    import os
-    import time
-
-    from . import _wire
-
-    comm = comm or _wire.Comm(group)
-    rank, world = comm.rank, comm.world
-    if segment_factory is None:
-        segment_factory = _default_segment_factory()
-    if ranges is None:
-        ranges = segment_ranges(prob, world)
-        my_slice = prob.slice_columns(*ranges[rank]) if ranges[rank] is not None else None
-    last_active = max(r for r in range(world) if ranges[r] is not None)
-    T = 1 << (2 * (my_slice.n_trios if my_slice is not None else 0))
-    marks = [("start", time.perf_counter())]
-    mark = lambda name: marks.append((name, time.perf_counter()))
-    seg, mine = None, ranges[rank]
-
-    def phase(fn):
-        """Run a rank-local step; returns (status, result)."""
-        try:
-            return (0, ""), fn()
-        except Exception as e:  # noqa: BLE001 - reported to every rank below
-            return _wire.status_of(e), None
-
-    try:
-        status, seg = phase(lambda: segment_factory(my_slice, mine[0] > 0) if mine is not None else None)
-        if _wire.raise_first_error(comm.all_status(*status), "create"):
-            return False, None
-        mark("create")
-        status, matrix = phase(lambda: seg.transfer() if seg else None)
-        mark("transfer")
-        T_all = max(comm.lengths(T))  # ranks without columns do not know T
-        width = 4 * T_all * T_all
-        states = comm.all_status(*status, payload=None if matrix is None else np.ascontiguousarray(matrix, np.uint32), payload_width=width)
-        _wire.raise_first_error(states, "transfer")
-        matrices = [None if pl is None else pl.view(np.uint32).reshape(T_all, T_all).copy() for _, _, pl in states]
-        mark("gather matrices")
-        status, out_vec = phase(lambda: seg.sweep(segment_inputs(matrices)[rank]) if seg else None)
-        _wire.raise_first_error(comm.all_status(*status), "sweep")
-        mark("sweep")
-        status, ex = phase(lambda: seg.exits(rank == last_active) if seg else None)
-        states = comm.all_status(*status, payload=None if ex is None else np.ascontiguousarray(ex, np.uint32), payload_width=4 * T_all)
-        _wire.raise_first_error(states, "exits")
-        exits = [None if pl is None else pl.view(np.uint32).copy() for _, _, pl in states]
-        mark("exits + gather")
-        entry = segment_entries(exits)[rank]
-        status, part = phase(lambda: seg.finish(entry) if seg else None)
-        _wire.raise_first_error(comm.all_status(*status), "finish")
-        mark("finish")
-    finally:
-        if seg is not None:
-            seg.close()
-    rows = comm.gather_rows(_wire.encode_solution(part, tag=rank) if part is not None else np.zeros(0, np.uint8))
-    mark("gather results")
-    if timings is not None:
-        timings.update({name: (t - t0) * 1e3 for (name, t), (_, t0) in zip(marks[1:], marks[:-1])})
-    if rank == 0 and os.environ.get("WHMEC_TIMING"):
-        print("[whmec] pedigree segments, rank 0: " + ", ".join(
-            "%s %.1f ms" % (name, (t - t0) * 1e3) for (name, t), (_, t0) in zip(marks[1:], marks[:-1])), flush=True)
-    if rank != 0:
-        return True, None
-    parts = [(r, _wire.decode_solution(row)[0]) for r, row in enumerate(rows) if row.size]
-    return True, merge_block_solutions(prob, [ranges[r] for r, _ in parts], [sol for _, sol in parts], cost=int(parts[-1][1].cost))
-
-
-def solve_sharded(prob: Optional[FlatProblem], solver: Optional[Callable[[FlatProblem], FlatSolution]] = None,
-                  group=None, segment_factory=None, comm=None, timings: Optional[dict] = None) -> Optional[FlatSolution]:
-    """Solve `prob` (given on rank 0; other ranks pass None) on all ranks of `group`.
-
-    Rank 0 cuts the problem and SCATTERS the pieces — a rank receives only the columns and reads it works on (the
-    "trivial broadcast of the block list" of the north_star, without shipping every rank the whole ReadSet): the blocks of
-    its share for a single individual, its segment of the table for a pedigree.  The pieces travel as flat byte rows through
-    tensor collectives (`_wire`), the per-block results come back the same way.  Returns the merged solution on rank 0 and
-    None elsewhere; an error on any rank is raised on every rank.  `solver` / `segment_factory` default to the CUDA path on
-    this rank's current device; tests inject CPU stand-ins to exercise the sharding logic with gloo.  `timings` (optional
-    dict) receives this rank's per-phase wall times in ms."""
-    import time
-
-    from . import _wire
-
-    if solver is None:
-        import torch
-
-        from . import _lib
-
-        device = torch.cuda.current_device()
-        solver = lambda p: _lib.solve(p, device=device)[0]
-    comm = comm or _wire.Comm(group)
-    rank, world = comm.rank, comm.world
-    t0 = time.perf_counter()
-    rows = None
-    MODE = {"whole": 0, "blocks": 1, "segments": 2}
-    if rank == 0:
-        spans = _read_spans(prob) if prob.n_reads else None
-        mode, ranges = plan_parts(prob, world, spans=spans)
-        if mode == "segments":
-            flat = np.array([MODE["segments"]] + [x for r in ranges for x in (r if r is not None else (0, 0))], np.int64)
-            rows = [[flat.view(np.uint8)] + ([enc] if enc is not None else []) for enc in _wire.encode_problem_slices(prob, ranges)]
-        elif mode == "whole":
-            rows = [[np.array([MODE["whole"]], np.int64).view(np.uint8)]] * world
-        else:
-            # every rank gets ONE sub-problem: a contiguous run of whole blocks with about 1 / world of the DP cells (one
-            # whmec_solve per rank sweeps all its chains together; block-by-block calls would be launch-latency bound)
-            rows = [[np.array([MODE["blocks"]], np.int64).view(np.uint8)] + ([enc] if enc is not None else [])
-                    for enc in _wire.encode_problem_slices(prob, ranges)]
-    t1 = time.perf_counter()
-    pieces = _wire.separate(comm.scatter_rows(rows))
-    head = pieces[0].view(np.int64)
-    mode = int(head[0])
-    t2 = time.perf_counter()
-    if timings is not None:
-        timings.update({"cut + encode": (t1 - t0) * 1e3, "scatter": (t2 - t1) * 1e3})
-    if mode == MODE["segments"]:
-        ranges = [None if head[1 + 2 * r] == head[2 + 2 * r] else (int(head[1 + 2 * r]), int(head[2 + 2 * r])) for r in range(world)]
-        piece = _wire.decode_problem(pieces[1])[0] if len(pieces) > 1 else None
-        handled, sol = solve_pedigree_sharded(prob, segment_factory, group, ranges=ranges, my_slice=piece, comm=comm, timings=timings)
-        if handled:
-            return sol
-        mode = MODE["whole"]  # some segment is outside the two-pass scheme: the whole table on rank 0's GPU
-    if mode == MODE["whole"]:
-        sol, err = None, None
-        if rank == 0:
-            try:
-                sol = solver(prob)
-            except Exception as e:  # noqa: BLE001
-                err = e
-        _wire.raise_first_error(comm.all_status(*_wire.status_of(err)), "solve")
-        return sol
-    mine, err = [], None
-    try:
-        for row in pieces[1:]:
-            sub, r, lo = _wire.decode_problem(row)
-            mine.append(_wire.encode_solution(solver(sub), tag=lo, extra=np.array([sub.n_cols], np.uint32)))
-    except Exception as e:  # noqa: BLE001 - e.g. more active reads than supported, CUDA out of memory
-        err = e
-    t3 = time.perf_counter()
-    _wire.raise_first_error(comm.all_status(*_wire.status_of(err)), "solve")
-    gathered = comm.gather_rows(_wire.join(mine))  # per-rank super-reads back to rank 0
-    t4 = time.perf_counter()
-    if timings is not None:
-        timings.update({"solve": (t3 - t2) * 1e3, "gather": (t4 - t3) * 1e3})
-    if rank != 0:
-        return None
-    parts = []
-    for row in gathered:
-        for enc in _wire.separate(row):
-            sol, lo, extra = _wire.decode_solution(enc)
-            parts.append(((lo, lo + int(extra[0])), sol))
-    parts.sort(key=lambda p: p[0][0])
-    out = merge_block_solutions(prob, [sp for sp, _ in parts], [sol for _, sol in parts])
-    if timings is not None:
-        timings["merge"] = (time.perf_counter() - t4) * 1e3
-    return out
 
 
 def _scaled(vec: np.ndarray) -> np.ndarray:
@@ -433,159 +239,53 @@ def genotype_segment_inputs(matrices: Sequence[Optional[np.ndarray]]) -> Tuple[L
     return alphas, betas
 
 
-def _default_genotype_segment_factory():
-    import torch
-
-    from . import _lib
-
-    device = torch.cuda.current_device()
-    return lambda p, continues, continued: _lib.GenotypeSegment(p, continues, continued, device=device)
-
-
-def genotype_pedigree_segments(prob: FlatProblem, n_segments: int, segment_factory=None) -> np.ndarray:
-    """The multi-GPU pedigree genotyping scheme with all `n_segments` segments driven by ONE process on one device, in the
-    order the ranks would run them: transfer matrices, the fold, then every segment's run.  Returns [n_ind, n_cols, 3]."""
-    if segment_factory is None:
-        segment_factory = _default_genotype_segment_factory()
-    ranges = segment_ranges(prob, n_segments)
-    out = np.zeros((prob.n_ind, prob.n_cols, 3), np.float64)
-    segs = []
-    try:
-        for r in ranges:
-            segs.append(None if r is None else segment_factory(prob.slice_columns(*r), r[0] > 0, r[1] < prob.n_cols))
-        alphas, betas = genotype_segment_inputs([sg.transfer() if sg else None for sg in segs])
-        for r, sg, a, b in zip(ranges, segs, alphas, betas):
-            if sg:
-                out[:, r[0]:r[1], :] = sg.run(a, b)
-    finally:
-        for sg in segs:
-            if sg:
-                sg.close()
-    return out
-
-
-def genotype_sharded(prob: Optional[FlatProblem], solver: Optional[Callable[[FlatProblem], np.ndarray]] = None,
-                     group=None, comm=None, segment_factory=None) -> Optional[np.ndarray]:
-    """Genotype likelihoods (`whmec_genotype`, the reference's GenotypeDPTable) of `prob` (given on rank 0; other ranks
-    pass None) on all ranks of `group`; returns [n_ind, n_cols, 3] on rank 0, None elsewhere.
-
-    Without transmission values every DP-independent chain is a forward-backward table of its own (a chain boundary hands
-    over one number, which cancels in each column's normalisation), so a single individual shards like the phasing DP:
-    every rank takes a contiguous run of whole chains balanced by DP cells, no collective on the data path, likelihoods
-    gathered on rank 0.  A pedigree with two chains or more is cut into segments of whole chains (`segment_ranges`), one
-    per rank: one all-gather of the T x T transfer matrices, the fold (`genotype_segment_inputs`), every rank runs its
-    segment, likelihoods gathered on rank 0.  A pedigree of one chain runs on rank 0's GPU, as does the whole table when
-    any rank's segment is refused as unsupported in any phase.  A refusal of the table on one GPU is raised as Unsupported on
-    every rank.  `solver` / `segment_factory` default to the CUDA path on this rank's
-    current device.  Errors are raised on every rank."""
-    from . import _wire
-
-    if solver is None:
-        import torch
-
-        from . import _lib
-
-        device = torch.cuda.current_device()
-        solver = lambda p: _lib.genotype(p, device=device)[0]
-    comm = comm or _wire.Comm(group)
-    rank, world = comm.rank, comm.world
-    rows = None
-    if rank == 0:
-        plan, ranges = plan_parts(prob, world, genotype=True)
-        if plan == "whole":
-            rows = [_wire.join([np.array([0, 0, 0, 0], np.int64).view(np.uint8)])] * world
-        else:  # every rank receives only its run of chains or its segment of the table
-            rows = []
-            for r in ranges:
-                lo, hi = r if r is not None else (0, 0)
-                rows.append(_wire.join([np.array([2 if plan == "segments" else 1, lo, hi, prob.n_cols], np.int64).view(np.uint8)] +
-                                       ([_wire.encode_problem(prob.slice_columns(lo, hi), lo=lo)] if hi > lo else [])))
-    pieces = _wire.separate(comm.scatter_rows(rows))
-    mode, lo, hi, n_cols = (int(x) for x in pieces[0].view(np.int64))
-    out, err = None, None
-    if mode == 2:
-        handled, out = _genotype_segment_rank(pieces[1] if len(pieces) > 1 else None, lo, hi, n_cols, comm, segment_factory)
-        if not handled:
-            mode = 0
-    try:
-        if mode == 0:
-            out = solver(prob) if rank == 0 else None
-        elif mode == 1 and len(pieces) > 1:
-            out = np.ascontiguousarray(solver(_wire.decode_problem(pieces[1])[0]), np.float64)
-    except Exception as e:  # noqa: BLE001
-        err = e
-    if mode != 2:
-        states = comm.all_status(*_wire.status_of(err))
-        if _wire.raise_first_error(states, "genotype"):  # refused as unsupported: raised on every rank, as the one-GPU call raises it
-            from ._abi import Unsupported
-
-            raise Unsupported(next(text for kind, text, _ in states if kind == 1))
-    if mode == 0:
-        return out
-    head = np.array([lo, hi], np.int64).view(np.uint8)
-    gathered = comm.gather_rows(_wire.join([head, out.reshape(-1).view(np.uint8)]) if out is not None else np.zeros(0, np.uint8))
-    if rank != 0:
-        return None
-    full = np.zeros((prob.n_ind, prob.n_cols, 3), np.float64)
-    for row in gathered:
-        parts = _wire.separate(row)
-        if parts:
-            lo, hi = (int(x) for x in parts[0].view(np.int64))
-            full[:, lo:hi, :] = parts[1].view(np.float64).reshape(prob.n_ind, hi - lo, 3)
-    return full
-
-
-def _genotype_segment_rank(row: Optional[np.ndarray], lo: int, hi: int, n_cols: int, comm, segment_factory=None
-                           ) -> Tuple[bool, Optional[np.ndarray]]:
-    """This rank's part of `genotype_sharded` for a pedigree cut into segments: `row` holds its columns [lo, hi) of the
-    n_cols (None: no columns).  Returns (True, its likelihoods or None), or (False, None) on every rank when some rank
-    reports 'unsupported' in any phase (the caller then genotypes the whole table on rank 0's GPU, which gives what the
-    single-GPU call gives, its refusal included).  Every phase reports its status in the all-gather that follows
-    it, so an error on one rank is raised on every rank."""
-    from . import _wire
-
-    if segment_factory is None:
-        segment_factory = _default_genotype_segment_factory()
-    my_slice = _wire.decode_problem(row)[0] if row is not None else None
-    T = 1 << (2 * (my_slice.n_trios if my_slice is not None else 0))
-    seg = None
-
-    def phase(fn):
-        try:
-            return (0, ""), fn()
-        except Exception as e:  # noqa: BLE001 - reported to every rank below
-            return _wire.status_of(e), None
-
-    try:
-        status, seg = phase(lambda: segment_factory(my_slice, lo > 0, hi < n_cols) if my_slice is not None else None)
-        if _wire.raise_first_error(comm.all_status(*status), "create"):
-            return False, None
-        status, matrix = phase(lambda: seg.transfer() if seg else None)
-        T_all = max(comm.lengths(T))  # ranks without columns do not know T
-        states = comm.all_status(*status, payload=None if matrix is None else np.ascontiguousarray(matrix, np.float64),
-                                 payload_width=8 * T_all * T_all)
-        if _wire.raise_first_error(states, "transfer"):
-            return False, None
-        matrices = [None if pl is None else pl.view(np.float64).reshape(T_all, T_all).copy() for _, _, pl in states]
-        alphas, betas = genotype_segment_inputs(matrices)
-        status, out = phase(lambda: np.ascontiguousarray(seg.run(alphas[comm.rank], betas[comm.rank]), np.float64) if seg else None)
-        # e.g. a segment whose backward tables find no room on its device: no rank may return a partial table
-        if _wire.raise_first_error(comm.all_status(*status), "run"):
-            return False, None
-    finally:
-        if seg is not None:
-            seg.close()
-    return True, out
-
-
-# ---- one process, several devices ---------------------------------------------------------------------------------
+# ---- the schemes and their executors ------------------------------------------------------------------------------
 #
-# The same cuts and folds as the distributed drivers above, for a caller that is a single process (`whatshap phase` and
-# `whatshap genotype` build one table at a time): one host thread per distinct device runs that device's parts through the
-# C ABI, which is re-entrant, sets the device on the calling thread and releases the GIL (ctypes); the folds between
-# phases run on the calling thread.
+# A table cut by `plan_parts` runs as parts in column order, phase by phase.  An executor runs one phase over every part and
+# returns one result per part (None for a part without columns): after a shared phase every participant holds every part's
+# result, after the others only the part's owner does.  `_Local` runs the parts one after another in one process, `_Threads`
+# on one host thread per device, `_Ranks` one part per rank of a process group.  The segment schemes of the two DPs
+# (`_phasing_segments`, `_genotype_segments`) and the runs of blocks or of the whole table (`_run_parts`) are written once
+# against that interface; a segment refused as unsupported sends the whole table to the first device, except on `_Local`,
+# which raises the refusal.
 
-ENV_DEVICES = "WHMEC_DEVICES"
+
+class _Local:
+    """One process, one device: the parts in column order, an error or a refusal raised at once."""
+
+    def __init__(self, prob: FlatProblem, ranges):
+        self.prob, self.n_cols, self.ranges = prob, prob.n_cols, list(ranges)
+
+    def piece(self, i: int) -> FlatProblem:
+        """Part i's columns of the table."""
+        r = self.ranges[i]
+        return self.prob if r == (0, self.n_cols) else self.prob.slice_columns(*r)
+
+    def on(self, i: int) -> tuple:
+        """The trailing arguments that put a call on part i's device (none: this process's current device)."""
+        return ()
+
+    def run(self, step, name: str, share=None, then: Optional[str] = None) -> list:
+        """`step(i)` for every part i with columns.  `share` = (dtype, number of T-long dimensions) of a result every
+        participant receives; `name` (and `then`, after the exchange of a shared result) name the phase's times."""
+        return [None if r is None else step(i) for i, r in enumerate(self.ranges)]
+
+    def close(self, segs) -> None:
+        for sg in segs:
+            if sg is not None:
+                sg.close()
+
+    def collect(self, done: list, codec, name: str) -> Optional[list]:
+        """Every part's result where the table is assembled; None on the other ranks.  `codec` = (encode, decode) of a result
+        that travels between ranks."""
+        return done
+
+    def mark(self, name: str) -> None:
+        pass
+
+    def whole(self) -> None:
+        """From here on the table is one part, on the first device (rank 0)."""
+        self.ranges = [(0, self.n_cols)] + [None] * (len(self.ranges) - 1)
 
 
 def _run_on_devices(devices: Sequence[int], jobs: Sequence[Optional[Callable[[], object]]]) -> Tuple[list, list]:
@@ -617,25 +317,273 @@ def _run_on_devices(devices: Sequence[int], jobs: Sequence[Optional[Callable[[],
     return results, errors
 
 
-def _raise_first(errors: Sequence[Optional[BaseException]], refusals_fall_back: bool) -> bool:
-    """Raises the error of the part with the lowest column (the parts are in column order).  With `refusals_fall_back` a
-    refusal (Unsupported) is not raised but reported: returns True if some part was refused, as `_wire.raise_first_error`
-    does for the ranks of the distributed drivers."""
-    from ._abi import Unsupported
+def _raise_first(errors: Sequence[Optional[BaseException]], refusals_last: bool) -> None:
+    """Raises the error of the part with the lowest column (the parts are in column order); with `refusals_last` a refusal
+    (Unsupported) only when no part failed otherwise."""
+    for e in sorted((e for e in errors if e is not None), key=lambda e: refusals_last and isinstance(e, Unsupported)):
+        raise e
 
-    for e in errors:
-        if e is not None and not (refusals_fall_back and isinstance(e, Unsupported)):
-            raise e
-    return any(isinstance(e, Unsupported) for e in errors)
+
+class _Threads(_Local):
+    """One process, part i on `devices[i]`, one host thread per distinct device (`_run_on_devices`).  An error is raised after
+    every thread has been joined: that of the part with the lowest column, where `refusals_last` (segment mode) puts the
+    refusals after every other error."""
+
+    def __init__(self, prob: FlatProblem, ranges, devices: List[int], refusals_last: bool):
+        super().__init__(prob, ranges or [None] * len(devices))
+        self.devices, self.refusals_last = devices, refusals_last
+
+    def on(self, i: int) -> tuple:
+        return (self.devices[i],)
+
+    def run(self, step, name: str, share=None, then: Optional[str] = None) -> list:
+        done, errors = _run_on_devices(self.devices, [None if r is None else (lambda i=i: step(i)) for i, r in enumerate(self.ranges)])
+        _raise_first(errors, self.refusals_last)
+        return done
+
+    def close(self, segs) -> None:
+        _run_on_devices(self.devices, [None if sg is None else sg.close for sg in segs])  # on the segment's own device thread
+
+
+_MODES = ("whole", "blocks", "segments")
+
+
+class _Ranks(_Local):
+    """One process per rank of `comm`, rank r holding part r.  Rank 0 cuts `prob` (`plan_parts`) and scatters to every rank one
+    row: the header [mode, n_cols, lo_0, hi_0, lo_1, hi_1, ...] (lo = hi: no columns) and the rank's columns
+    (`_wire.encode_problem_slices`, written straight into the page-locked send buffer).  Every phase ends in one `all_status`
+    that carries the shared results, so an error on one rank is raised on every rank, and a refusal as Unsupported on every
+    rank.  The results are gathered to rank 0.  `times` (the caller's `timings` if given) receives the ms of every phase."""
+
+    def __init__(self, comm, prob: Optional[FlatProblem], genotype: bool, timings: Optional[dict]):
+        self.comm, self.prob, self.rank = comm, prob, comm.rank
+        self.times = timings if timings is not None else {}
+        self.T = None
+        self._t = time.perf_counter()
+        rows = None
+        if self.rank == 0:
+            mode, ranges = plan_parts(prob, comm.world, genotype, spans=_read_spans(prob) if prob.n_reads else None)
+            ranges = ranges or [None] * comm.world
+            head = np.array([_MODES.index(mode), prob.n_cols] + [x for r in ranges for x in (r or (0, 0))], np.int64).view(np.uint8)
+            rows = [[head] + ([enc] if enc is not None else []) for enc in _wire.encode_problem_slices(prob, ranges)]
+        self.mark("cut + encode")
+        pieces = _wire.separate(comm.scatter_rows(rows))
+        head = pieces[0].view(np.int64)
+        self.mode, self.n_cols = _MODES[int(head[0])], int(head[1])
+        self.ranges = [None if lo == hi else (int(lo), int(hi)) for lo, hi in head[2:].reshape(-1, 2)]
+        self.mine = _wire.decode_problem(pieces[1])[0] if len(pieces) > 1 else None
+        self.mark("scatter")
+
+    def piece(self, i: int) -> FlatProblem:
+        return self.prob if self.prob is not None and self.ranges[i] == (0, self.n_cols) else self.mine
+
+    def run(self, step, name: str, share=None, then: Optional[str] = None) -> list:
+        result, status = None, (0, "")
+        if self.ranges[self.rank] is not None:
+            try:
+                result = step(self.rank)
+            except Exception as e:  # noqa: BLE001 - reported to every rank below
+                status = _wire.status_of(e)
+        if then:
+            self.mark(name)
+        if share is None:
+            states = self.comm.all_status(*status)
+        else:
+            dtype, dims = share
+            if self.T is None:  # ranks without columns do not know T
+                self.T = max(self.comm.lengths(4 ** self.mine.n_trios if self.mine is not None else 0))
+            states = self.comm.all_status(*status, payload=None if result is None else np.ascontiguousarray(result, dtype),
+                                          payload_width=np.dtype(dtype).itemsize * self.T ** dims)
+        self.mark(then or name)
+        if _wire.raise_first_error(states, name):
+            raise Unsupported(next(text for kind, text, _ in states if kind == 1))
+        if share is None:
+            return [result if r == self.rank else None for r in range(len(self.ranges))]
+        return [None if pl is None else pl.view(dtype).reshape((self.T,) * dims).copy() for _, _, pl in states]
+
+    def collect(self, done: list, codec, name: str) -> Optional[list]:
+        if any(self.ranges[1:]):  # (else only rank 0 holds columns: the whole table, nothing to gather)
+            mine = done[self.rank]
+            rows = self.comm.gather_rows(codec[0](mine) if mine is not None else np.zeros(0, np.uint8))
+            done = None if rows is None else [codec[1](row) if row.size else None for row in rows]
+        self.mark(name)
+        return done if self.rank == 0 else None
+
+    def mark(self, name: str) -> None:
+        now = time.perf_counter()
+        self.times[name] = (now - self._t) * 1e3
+        self._t = now
+
+
+def _current(fn):
+    """`fn(..., device=d)` on this process's current CUDA device d."""
+    import torch
+
+    device = torch.cuda.current_device()
+    return lambda *args: fn(*args, device=device)
+
+
+def _run_parts(ex: _Local, mode: str, solver, segments) -> Tuple[list, str]:
+    """Every part's result and the mode that ran: `segments()` in segment mode, else `solver(part, *device)` on every run of
+    blocks, or on the whole table (whole mode, and segment mode when some segment is refused as unsupported in any phase)."""
+    if mode == "segments":
+        try:
+            return segments(), mode
+        except Unsupported:  # no part may leave its columns empty
+            mode = "whole"
+    if mode == "whole":
+        ex.whole()
+    return ex.run(lambda i: solver(ex.piece(i), *ex.on(i)), "solve"), mode
+
+
+def _phasing_segments(ex: _Local, factory) -> list:
+    """The phasing segments of `ex`: create (`factory(slice, continues, *device)`), transfer (T x T, shared), `segment_inputs`,
+    sweep, exits (shared), `segment_entries`, finish.  Returns every part's (solution, statistics)."""
+    segs: list = [None] * len(ex.ranges)
+    last = max(i for i, r in enumerate(ex.ranges) if r is not None)
+
+    def create(i):
+        segs[i] = factory(ex.piece(i), ex.ranges[i][0] > 0, *ex.on(i))
+
+    try:
+        ex.run(create, "create")
+        inputs = segment_inputs(ex.run(lambda i: segs[i].transfer(), "transfer", (np.uint32, 2), then="gather matrices"))
+        ex.run(lambda i: segs[i].sweep(inputs[i]), "sweep")
+        entries = segment_entries(ex.run(lambda i: segs[i].exits(i == last), "exits + gather", (np.uint32, 1)))
+        return ex.run(lambda i: (segs[i].finish(entries[i]), _segment_stats(segs[i])), "finish")
+    finally:
+        ex.close(segs)
+
+
+def _merged(ex: _Local, prob: FlatProblem, done: list, mode: str) -> Tuple[Optional[FlatSolution], Optional[list]]:
+    """The parts' solutions merged in column order, and every part's statistics; (None, None) on ranks other than 0.  The
+    last segment's cost is the table's; the costs of runs of blocks add."""
+    parts = ex.collect(done, _SOLUTIONS, "gather results" if mode == "segments" else "gather")
+    if parts is None:
+        return None, None
+    held = [(r, p[0]) for r, p in zip(ex.ranges, parts) if p is not None]
+    sol = merge_block_solutions(prob, [r for r, _ in held], [s for _, s in held], cost=int(held[-1][1].cost) if mode == "segments" else None)
+    if mode != "segments":
+        ex.mark("merge")
+    return sol, [None if p is None else dict(p[1] or {}) for p in parts]
+
+
+def _genotype_segments(ex: _Local, factory) -> list:
+    """The genotyping segments of `ex`: create (`factory(slice, continues, continued, *device)`), transfer (T x T, shared),
+    `genotype_segment_inputs`, run.  Returns every part's (likelihoods, {"transfer": statistics, "run": statistics})."""
+    segs: list = [None] * len(ex.ranges)
+
+    def create(i):
+        lo, hi = ex.ranges[i]
+        segs[i] = factory(ex.piece(i), lo > 0, hi < ex.n_cols, *ex.on(i))
+
+    try:
+        ex.run(create, "create")
+        alphas, betas = genotype_segment_inputs(ex.run(lambda i: segs[i].transfer(), "transfer", (np.float64, 2)))
+        transfers = [_segment_stats(sg) for sg in segs]
+        return ex.run(lambda i: (segs[i].run(alphas[i], betas[i]), {"transfer": transfers[i], "run": _segment_stats(segs[i])}), "run")
+    finally:
+        ex.close(segs)
+
+
+def _likelihoods(ex: _Local, prob: FlatProblem, done: list) -> Tuple[Optional[np.ndarray], Optional[list]]:
+    """The parts' likelihoods written into [n_ind, n_cols, 3], and every part's statistics; (None, None) on ranks other than 0."""
+    parts = ex.collect(done, _LIKELIHOODS, "gather")
+    if parts is None:
+        return None, None
+    out = np.zeros((prob.n_ind, prob.n_cols, 3), np.float64)
+    for r, p in zip(ex.ranges, parts):
+        if p is not None:
+            out[:, r[0]:r[1], :] = np.reshape(p[0], (prob.n_ind, r[1] - r[0], 3))
+    return out, [None if p is None else dict(p[1] or {}) for p in parts]
+
+
+_SOLUTIONS = (lambda part: _wire.encode_solution(part[0]), lambda row: (_wire.decode_solution(row)[0], None))
+_LIKELIHOODS = (lambda part: np.ascontiguousarray(part[0], np.float64).reshape(-1).view(np.uint8), lambda row: (row.view(np.float64), None))
+
+
+def solve_pedigree_segments(prob: FlatProblem, n_segments: int, segment_factory=None) -> FlatSolution:
+    """The multi-GPU pedigree scheme with all `n_segments` segments driven by ONE process on one
+    device, in the order the ranks would run them -- the single-GPU check of `whmec_segment_*`
+    (tests/test_gpu_sharded.py) and of this module's folding logic."""
+    from . import _lib
+
+    ex = _Local(prob, segment_ranges(prob, n_segments))
+    return _merged(ex, prob, _phasing_segments(ex, segment_factory or _current(_lib.Segment)), "segments")[0]
+
+
+def solve_sharded(prob: Optional[FlatProblem], solver: Optional[Callable[[FlatProblem], FlatSolution]] = None,
+                  group=None, segment_factory=None, comm=None, timings: Optional[dict] = None) -> Optional[FlatSolution]:
+    """Solve `prob` (given on rank 0; other ranks pass None) on all ranks of `group`.
+
+    Rank 0 cuts the problem and SCATTERS the pieces — a rank receives only the columns and reads it works on (the
+    "trivial broadcast of the block list" of the north_star, without shipping every rank the whole ReadSet): the blocks of
+    its share for a single individual, its segment of the table for a pedigree.  The pieces travel as flat byte rows through
+    tensor collectives (`_wire`), the per-block results come back the same way.  Returns the merged solution on rank 0 and
+    None elsewhere; an error on any rank is raised on every rank, and so is a refusal (Unsupported) of a run of blocks or of
+    the whole table.  A pedigree of one chain runs on rank 0's GPU, as does the whole table when any rank's segment is refused
+    as unsupported in any phase.  `solver` / `segment_factory` default to the CUDA path on this rank's current device; tests
+    inject CPU stand-ins to exercise the sharding logic with gloo.  `timings` (optional dict) receives this rank's per-phase
+    wall times in ms."""
+    from . import _lib
+
+    if solver is None:
+        solve = _current(_lib.solve)
+        solver = lambda p: solve(p)[0]  # noqa: E731
+    ex = _Ranks(comm or _wire.Comm(group), prob, False, timings)
+    done, mode = _run_parts(ex, ex.mode, lambda p: (solver(p), None), lambda: _phasing_segments(ex, segment_factory or _current(_lib.Segment)))
+    sol = _merged(ex, prob, done, mode)[0]
+    if ex.rank == 0 and mode == "segments" and os.environ.get("WHMEC_TIMING"):
+        print("[whmec] pedigree segments, rank 0: " + ", ".join("%s %.1f ms" % kv for kv in list(ex.times.items())[2:]), flush=True)
+    return sol
+
+
+def genotype_pedigree_segments(prob: FlatProblem, n_segments: int, segment_factory=None) -> np.ndarray:
+    """The multi-GPU pedigree genotyping scheme with all `n_segments` segments driven by ONE process on one device, in the
+    order the ranks would run them: transfer matrices, the fold, then every segment's run.  Returns [n_ind, n_cols, 3]."""
+    from . import _lib
+
+    ex = _Local(prob, segment_ranges(prob, n_segments))
+    return _likelihoods(ex, prob, _genotype_segments(ex, segment_factory or _current(_lib.GenotypeSegment)))[0]
+
+
+def genotype_sharded(prob: Optional[FlatProblem], solver: Optional[Callable[[FlatProblem], np.ndarray]] = None,
+                     group=None, comm=None, segment_factory=None) -> Optional[np.ndarray]:
+    """Genotype likelihoods (`whmec_genotype`, the reference's GenotypeDPTable) of `prob` (given on rank 0; other ranks
+    pass None) on all ranks of `group`; returns [n_ind, n_cols, 3] on rank 0, None elsewhere.
+
+    Without transmission values every DP-independent chain is a forward-backward table of its own (a chain boundary hands
+    over one number, which cancels in each column's normalisation), so a single individual shards like the phasing DP:
+    every rank takes a contiguous run of whole chains balanced by DP cells, no collective on the data path, likelihoods
+    gathered on rank 0.  A pedigree with two chains or more is cut into segments of whole chains (`segment_ranges`), one
+    per rank: one all-gather of the T x T transfer matrices, the fold (`genotype_segment_inputs`), every rank runs its
+    segment, likelihoods gathered on rank 0.  A pedigree of one chain runs on rank 0's GPU, as does the whole table when
+    any rank's segment is refused as unsupported in any phase.  A refusal of the table on one GPU is raised as Unsupported on
+    every rank.  `solver` / `segment_factory` default to the CUDA path on this rank's
+    current device.  Errors are raised on every rank."""
+    from . import _lib
+
+    if solver is None:
+        genotype = _current(_lib.genotype)
+        solver = lambda p: genotype(p)[0]  # noqa: E731
+    ex = _Ranks(comm or _wire.Comm(group), prob, True, None)
+    done, _ = _run_parts(ex, ex.mode, lambda p: (solver(p), None), lambda: _genotype_segments(ex, segment_factory or _current(_lib.GenotypeSegment)))
+    return _likelihoods(ex, prob, done)[0]
+
+
+# ---- one process, several devices ---------------------------------------------------------------------------------
+#
+# The same cuts and schemes as the distributed drivers above, for a caller that is a single process (`whatshap phase` and
+# `whatshap genotype` build one table at a time): one host thread per distinct device runs that device's parts through the
+# C ABI, which is re-entrant, sets the device on the calling thread and releases the GIL (ctypes); the folds between
+# phases run on the calling thread.
+
+ENV_DEVICES = "WHMEC_DEVICES"
 
 
 def _segment_stats(seg) -> dict:
     st = getattr(seg, "stats", None)  # `_lib.Segment.stats()`, `_lib.GenotypeSegment.stats` (its last call)
     return dict(st() if callable(st) else st or {})
-
-
-def _whole_stats(n_cols: int, devices: Sequence[int], st) -> dict:
-    return {"mode": "whole", "devices": list(devices), "parts": [{"device": devices[0], "columns": (0, n_cols), "stats": dict(st or {})}]}
 
 
 def _part_stats(mode: str, devices: Sequence[int], ranges, stats) -> dict:
@@ -657,57 +605,11 @@ def solve_on_devices(prob: FlatProblem, devices: Sequence[int], solver=None, seg
     from . import _lib
 
     devices = [int(d) for d in devices]
-    solver = solver or _lib.solve
-    factory = segment_factory or _lib.Segment
     mode, ranges = plan_parts(prob, len(devices))
-    if mode == "blocks":
-        jobs = [None if r is None else (lambda r=r, d=d: solver(prob.slice_columns(*r), d)) for r, d in zip(ranges, devices)]
-        done, errors = _run_on_devices(devices, jobs)
-        _raise_first(errors, False)
-        parts = [(r, out) for r, out in zip(ranges, done) if r is not None]
-        return (merge_block_solutions(prob, [r for r, _ in parts], [out[0] for _, out in parts]),
-                _part_stats(mode, devices, ranges, [None if out is None else dict(out[1] or {}) for out in done]))
-    if mode == "segments":
-        done = _solve_segments(prob, devices, ranges, factory)
-        if done is not None:
-            return done
-    sol, st = solver(prob, devices[0])
-    return sol, _whole_stats(prob.n_cols, devices, st)
-
-
-def _solve_segments(prob: FlatProblem, devices: List[int], ranges, factory) -> Optional[Tuple[FlatSolution, dict]]:
-    """The segment mode of `solve_on_devices`; None when some segment is refused as unsupported."""
-    segs: list = [None] * len(ranges)
-    last_active = max(i for i, r in enumerate(ranges) if r is not None)
-
-    def phase(step):
-        """step(i, segment) on the thread of every part that holds a segment; True if one was refused."""
-        out, errors = _run_on_devices(devices, [None if sg is None else (lambda i=i, sg=sg: step(i, sg)) for i, sg in enumerate(segs)])
-        return out, _raise_first(errors, True)
-
-    try:
-        segs, errors = _run_on_devices(devices, [None if r is None else (lambda r=r, d=d: factory(prob.slice_columns(*r), r[0] > 0, d))
-                                                 for r, d in zip(ranges, devices)])
-        if _raise_first(errors, True):
-            return None
-        matrices, refused = phase(lambda i, sg: sg.transfer())
-        if refused:
-            return None
-        inputs = segment_inputs(matrices)
-        if phase(lambda i, sg: sg.sweep(inputs[i]))[1]:
-            return None
-        exits, refused = phase(lambda i, sg: sg.exits(i == last_active))
-        if refused:
-            return None
-        entries = segment_entries(exits)
-        done, refused = phase(lambda i, sg: (sg.finish(entries[i]), _segment_stats(sg)))
-        if refused:
-            return None
-    finally:
-        _run_on_devices(devices, [None if sg is None else sg.close for sg in segs])
-    parts = [(r, out[0]) for r, out in zip(ranges, done) if out is not None]
-    sol = merge_block_solutions(prob, [r for r, _ in parts], [s for _, s in parts], cost=int(parts[-1][1].cost))
-    return sol, _part_stats("segments", devices, ranges, [None if out is None else out[1] for out in done])
+    ex = _Threads(prob, ranges, devices, mode == "segments")
+    done, mode = _run_parts(ex, mode, solver or _lib.solve, lambda: _phasing_segments(ex, segment_factory or _lib.Segment))
+    sol, stats = _merged(ex, prob, done, mode)
+    return sol, _part_stats(mode, devices, ex.ranges, stats)
 
 
 def genotype_on_devices(prob: FlatProblem, devices: Sequence[int], solver=None, segment_factory=None) -> Tuple[np.ndarray, dict]:
@@ -721,55 +623,12 @@ def genotype_on_devices(prob: FlatProblem, devices: Sequence[int], solver=None, 
     from . import _lib
 
     devices = [int(d) for d in devices]
-    solver = solver or _lib.genotype
-    factory = segment_factory or _lib.GenotypeSegment
     mode, ranges = plan_parts(prob, len(devices), genotype=True)
-    if mode == "blocks":
-        jobs = [None if r is None else (lambda r=r, d=d: solver(prob.slice_columns(*r), d)) for r, d in zip(ranges, devices)]
-        done, errors = _run_on_devices(devices, jobs)
-        _raise_first(errors, False)
-        out = np.zeros((prob.n_ind, prob.n_cols, 3), np.float64)
-        for r, part in zip(ranges, done):
-            if r is not None:
-                out[:, r[0]:r[1], :] = part[0]
-        return out, _part_stats(mode, devices, ranges, [None if part is None else dict(part[1] or {}) for part in done])
-    if mode == "segments":
-        done = _genotype_segments(prob, devices, ranges, factory)
-        if done is not None:
-            return done
-    out, st = solver(prob, devices[0])
-    return out, _whole_stats(prob.n_cols, devices, st)
+    ex = _Threads(prob, ranges, devices, mode == "segments")
+    done, mode = _run_parts(ex, mode, solver or _lib.genotype, lambda: _genotype_segments(ex, segment_factory or _lib.GenotypeSegment))
+    out, stats = _likelihoods(ex, prob, done)
+    return out, _part_stats(mode, devices, ex.ranges, stats)
 
-
-def _genotype_segments(prob: FlatProblem, devices: List[int], ranges, factory) -> Optional[Tuple[np.ndarray, dict]]:
-    """The segment mode of `genotype_on_devices`; None when some segment is refused as unsupported."""
-    segs: list = [None] * len(ranges)
-    n = prob.n_cols
-
-    def phase(step):
-        out, errors = _run_on_devices(devices, [None if sg is None else (lambda i=i, sg=sg: step(i, sg)) for i, sg in enumerate(segs)])
-        return out, _raise_first(errors, True)
-
-    try:
-        segs, errors = _run_on_devices(devices, [None if r is None else (lambda r=r, d=d: factory(prob.slice_columns(*r), r[0] > 0, r[1] < n, d))
-                                                 for r, d in zip(ranges, devices)])
-        if _raise_first(errors, True):
-            return None
-        transfers, refused = phase(lambda i, sg: (sg.transfer(), _segment_stats(sg)))
-        if refused:
-            return None
-        alphas, betas = genotype_segment_inputs([None if t is None else t[0] for t in transfers])
-        runs, refused = phase(lambda i, sg: (sg.run(alphas[i], betas[i]), _segment_stats(sg)))
-        if refused:
-            return None
-    finally:
-        _run_on_devices(devices, [None if sg is None else sg.close for sg in segs])
-    out = np.zeros((prob.n_ind, n, 3), np.float64)
-    for r, run in zip(ranges, runs):
-        if run is not None:
-            out[:, r[0]:r[1], :] = run[0]
-    stats = [None if t is None else {"transfer": t[1], "run": run[1]} for t, run in zip(transfers, runs)]
-    return out, _part_stats("segments", devices, ranges, stats)
 
 
 def parse_devices(text: str) -> List[int]:
