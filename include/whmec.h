@@ -20,6 +20,7 @@
  *                             bound at whatshap/core.pyx:581-600  (sibling DP, SURVEY.md 8(f) rank 4)
  *   whmec_realign          <- ReadSetReader.detect_alleles_by_alignment  whatshap/variants.py:599-912 (allele detection
  *                             by re-alignment, the step that builds the ReadSet)
+ *   whmec_realign_kmerald  <- the same with use_kmerald=True  whatshap/variants.py:731-794, align.pyx:199-271
  *
  * Plain pointers and sizes only.  All input pointers are caller-owned host
  * memory, read-only, and need to stay valid only for the duration of the call.
@@ -334,7 +335,7 @@ int whmec_heuristic_batch(const whmec_problem *const *problems, whmec_heuristic_
 
 /* ---- Allele detection by re-alignment: ReadSetReader.detect_alleles_by_alignment(variants, restricted_genotypes, 0, alignment,
  * reference, overhang, use_affine, gap_start, gap_extend, default_mismatch) for many alignments in one call
- * (whatshap/variants.py:599-912, whatshap/_variants.pyx:10-81, whatshap/align.pyx:16-196).  kmer alignment is not covered.
+ * (whatshap/variants.py:599-912, whatshap/_variants.pyx:10-81, whatshap/align.pyx:16-196).  kmer alignment: whmec_realign_kmerald.
  * The host walks every CIGAR against the variant list (WHMEC_HOST_THREADS workers) and lists the (alignment, variant) items and
  * their alleles; the device builds each padded allele from the reference, strips common prefix and suffix, computes every
  * allele's distance and makes the call.  Work goes in chunks of items under the free HBM (or WHMEC_REALIGN_ARENA_BUDGET bytes). */
@@ -392,6 +393,41 @@ void whmec_realign_release(whmec_realign_output *out);
 int whmec_edit_distance_batch(uint32_t n, const uint64_t *query_off, const uint8_t *query, const uint64_t *target_off,
                               const uint8_t *target, double mismatch, int32_t gap_start, int32_t gap_extend, int64_t *unit_out,
                               int64_t *affine_out, int device, whmec_realign_stats *stats, char *err, size_t errlen);
+
+/* ---- Allele detection by k-mer re-alignment: detect_alleles_by_alignment(..., use_kmerald=True, kmerald_costs, kmer_size,
+ * kmerald_gappenalty, kmerald_window) (whatshap/variants.py:731-794, whatshap/align.pyx:199-271), `whatshap genotype
+ * --use-kmerald`.  Each covered, non-symbolic variant's query window (kmerald_window for the overhang) is cut into k-mers
+ * (enumerate_all_kmers) and aligned (kmer_align) against the k-mers of allele 0 and of the variant's alternative_allele; the
+ * smaller distance is called with quality 30, a tie or NaN gives no call.  The restricted genotypes, overhang, affine and the
+ * affine costs of whmec_realign_input are ignored. */
+typedef struct whmec_kmer_costs {
+    uint64_t n;                      /* < 2^32 */
+    const uint64_t *key;             /* [n], strictly ascending: (uint64_t)ref_kmer << 32 | read_kmer; read k-mer 0 stands for the
+                                        reference's -5 (the ref k-mer's default cost; a real k-mer is never 0) */
+    const float *cost;               /* [n]: float(value) as a float32 */
+} whmec_kmer_costs;
+
+typedef struct whmec_kmerald_params {
+    int32_t kmer_size;               /* 1..15 */
+    float gap_penalty;
+    int32_t window;                  /* int(kmerald_window), >= 0 */
+    const whmec_kmer_costs *costs;
+    const uint64_t *alt_off;         /* [n_variants + 1] into alt_bytes: each variant's alternative_allele (NULL in the batch) */
+    const uint8_t *alt_bytes;
+    const uint8_t *has_alt;          /* [n_variants]: 0 for a variant without alternative_allele (the reference raises on it) */
+} whmec_kmerald_params;
+
+/* Return codes, output, release (whmec_realign_release) and errors as whmec_realign; a covered, non-symbolic variant without
+ * alternative_allele is one more input on which the reference raises.  stats->short_jobs / long_jobs: one thread / one warp
+ * per allele alignment. */
+int whmec_realign_kmerald(const whmec_realign_input *in, const whmec_kmerald_params *params, int device, whmec_realign_output *out,
+                          whmec_realign_stats *stats, char *err, size_t errlen);
+
+/* kmer_align(enumerate_all_kmers(s1[i], k), enumerate_all_kmers(s2[i], k), costs, gap_penalty) for n pairs, as float32
+ * (params' alt fields are not used).  Return codes as whmec_realign. */
+int whmec_kmer_align_batch(uint32_t n, const uint64_t *s1_off, const uint8_t *s1, const uint64_t *s2_off, const uint8_t *s2,
+                           const whmec_kmerald_params *params, float *out, int device, whmec_realign_stats *stats, char *err,
+                           size_t errlen);
 
 #ifdef __cplusplus
 }

@@ -355,3 +355,25 @@ class CRealignStats(C.Structure):
 
     def as_dict(self) -> dict:
         return {name: getattr(self, name) for name, _ in self._fields_}
+
+
+class CKmerCosts(C.Structure):
+    """whmec_kmer_costs: the sorted costs table of k-mer realignment, keys (ref k-mer << 32 | read k-mer, 0 for -5)."""
+    _fields_ = [
+        ("n", C.c_uint64),
+        ("key", _u64p),
+        ("cost", C.POINTER(C.c_float)),
+    ]
+
+
+class CKmeraldParams(C.Structure):
+    """whmec_kmerald_params: k-mer size, gap penalty, window, costs and each variant's alternative_allele (CSR)."""
+    _fields_ = [
+        ("kmer_size", C.c_int32),
+        ("gap_penalty", C.c_float),
+        ("window", C.c_int32),
+        ("costs", C.POINTER(CKmerCosts)),
+        ("alt_off", _u64p),
+        ("alt_bytes", _u8p),
+        ("has_alt", _u8p),
+    ]

@@ -13,7 +13,7 @@ from typing import List, Optional, Sequence, Tuple, Union
 
 import numpy as np
 
-from ._abi import CHeuristicSolution, CProblem, CRealignInput, CRealignOutput, CRealignStats, CSolution, CStats, FlatProblem, FlatSolution, HeuristicSolution, raise_for
+from ._abi import CHeuristicSolution, CKmeraldParams, CProblem, CRealignInput, CRealignOutput, CRealignStats, CSolution, CStats, FlatProblem, FlatSolution, HeuristicSolution, raise_for
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("WHMEC_LIBRARY") or os.path.join(HERE, "libwhmec.so")  # WHMEC_LIBRARY: another build of the same library (A/B runs)
@@ -54,6 +54,8 @@ EXPORTS = (
     "whmec_realign",
     "whmec_realign_release",
     "whmec_edit_distance_batch",
+    "whmec_realign_kmerald",
+    "whmec_kmer_align_batch",
 )
 
 
@@ -138,8 +140,8 @@ def lib() -> C.CDLL:
 
 
 def realign_signatures(L: C.CDLL) -> C.CDLL:
-    """argtypes of whmec_realign, whmec_realign_release and whmec_edit_distance_batch on `L` (this library or a test build that
-    exports the same three symbols)."""
+    """argtypes of whmec_realign, whmec_realign_release, whmec_edit_distance_batch, whmec_realign_kmerald and
+    whmec_kmer_align_batch on `L` (this library or a test build that exports the same symbols; those it lacks are skipped)."""
     i64p = C.POINTER(C.c_int64)
     L.whmec_realign.argtypes = [C.POINTER(CRealignInput), C.c_int, C.POINTER(CRealignOutput), C.POINTER(CRealignStats), C.c_char_p, C.c_size_t]
     L.whmec_realign.restype = C.c_int
@@ -148,6 +150,14 @@ def realign_signatures(L: C.CDLL) -> C.CDLL:
     L.whmec_edit_distance_batch.argtypes = [C.c_uint32, C.POINTER(C.c_uint64), C.POINTER(C.c_uint8), C.POINTER(C.c_uint64), C.POINTER(C.c_uint8),
                                             C.c_double, C.c_int32, C.c_int32, i64p, i64p, C.c_int, C.POINTER(CRealignStats), C.c_char_p, C.c_size_t]
     L.whmec_edit_distance_batch.restype = C.c_int
+    if hasattr(L, "whmec_realign_kmerald"):
+        L.whmec_realign_kmerald.argtypes = [C.POINTER(CRealignInput), C.POINTER(CKmeraldParams), C.c_int, C.POINTER(CRealignOutput),
+                                            C.POINTER(CRealignStats), C.c_char_p, C.c_size_t]
+        L.whmec_realign_kmerald.restype = C.c_int
+        L.whmec_kmer_align_batch.argtypes = [C.c_uint32, C.POINTER(C.c_uint64), C.POINTER(C.c_uint8), C.POINTER(C.c_uint64), C.POINTER(C.c_uint8),
+                                             C.POINTER(CKmeraldParams), C.POINTER(C.c_float), C.c_int, C.POINTER(CRealignStats), C.c_char_p,
+                                             C.c_size_t]
+        L.whmec_kmer_align_batch.restype = C.c_int
     return L
 
 

@@ -1,6 +1,6 @@
-// Allele detection by re-alignment on the GPU (whmec_realign, DESIGN §4.11): the kernels of one chunk and its arena, uploads and
-// downloads (ra_run_chunk).  Per-job code: realign.h.  Compiled with -fmad=false: the affine recurrence must round one float
-// operation at a time, as align.pyx does.
+// Allele detection by re-alignment on the GPU (whmec_realign, DESIGN §4.11; k-mer mode, §4.12): the kernels of one chunk and its
+// arena, uploads and downloads (ra_run_chunk).  Per-job code: realign.h, kmerald.h.  Compiled with -fmad=false: the affine and
+// k-mer recurrences must round one float operation at a time, as align.pyx does.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -101,6 +101,67 @@ __global__ void __launch_bounds__(RA_BLOCK) ra_decide_kernel(const RaItem *items
     quality[i] = q;
 }
 
+// ---- k-mer mode (kmerald.h) ----------------------------------------------------------------------------------------------------
+
+// one thread per one-thread k-mer job
+__global__ void __launch_bounds__(RA_BLOCK) ka_short_kernel(RaBufs b, const RaItem *items, uint32_t item0, const RaJob *jobs, uint32_t n_jobs,
+                                                            KaParams p, float *dist) {
+    const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= n_jobs) return;
+    const RaJob jb = jobs[k];
+    if (jb.scratch != RA_NO_SCRATCH) return;
+    dist[k] = ka_short_job(b, items[jb.item - item0], jb.allele, p);
+}
+
+// one warp per longer k-mer job: lane 0 lists the k-mers into the job's scratch, every lane finds its rows' costs, then an
+// anti-diagonal wavefront over row bands, lane L one column behind lane L - 1
+__global__ void __launch_bounds__(RA_BLOCK) ka_long_kernel(RaBufs b, const RaItem *items, uint32_t item0, const RaJob *jobs, const uint32_t *list,
+                                                           uint32_t n_list, KaParams p, uint8_t *scratch, float *dist) {
+    const uint32_t lane = threadIdx.x & 31;
+    const uint32_t warps = gridDim.x * (blockDim.x / 32);
+    for (uint32_t w = (blockIdx.x * blockDim.x + threadIdx.x) / 32; w < n_list; w += warps) {
+        const uint32_t k = list[w];
+        const RaJob jb = jobs[k];
+        const RaItem it = items[jb.item - item0];
+        const RaSeq q = ra_query(b, it), t = ra_target(b, it, jb.allele);
+        const KaScratch s(scratch + jb.scratch, q.len, t.len);
+        uint32_t m = 0, n = 0, x = 0;
+        if (lane == 0) m = ka_kmers(t, p.k, s.a), n = ka_kmers(q, p.k, s.b);
+        m = __shfl_sync(FULL, m, 0);
+        n = __shfl_sync(FULL, n, 0);
+        __syncwarp();
+        float d = 0.0f;
+        if (ka_trim(s.a, s.b, m, n, x)) {
+            if (m == 0) {
+                d = p.gap * (float)n;
+            } else {
+                const uint32_t *a = s.a + x, *bq = s.b + x;
+                KaLane ln;
+                ln.init(m, lane, 32, a, s.row, s.S, p);
+                float out = 0.0f;
+                for (uint32_t st = 0; st < n + 31; ++st) {
+                    const float recv = __shfl_up_sync(FULL, out, 1);
+                    const int64_t j = (int64_t)st - lane + 1;
+                    if (ln.active() && j >= 1 && j <= n) out = ln.step(a, s.row, s.S, lane ? recv : p.gap * (float)j, bq[j - 1], p);
+                }
+                __syncwarp();
+                d = s.S[m];
+            }
+        }
+        if (lane == 0) dist[k] = d;
+    }
+}
+
+// one thread per item: the call from the distances of allele 0 and alternative_allele
+__global__ void __launch_bounds__(RA_BLOCK) ka_decide_kernel(const RaItem *items, uint32_t n_items, uint32_t job0, const float *dist, int32_t *call,
+                                                             int64_t *quality) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_items) return;
+    const RaItem it = items[i];
+    call[i] = ka_decide(dist[it.job0 - job0], dist[it.job0 - job0 + 1]);
+    quality[i] = 30;
+}
+
 #define RA_CUDA(expr)                                                 \
     do {                                                              \
         cudaError_t _e = (expr);                                      \
@@ -117,12 +178,51 @@ struct RaDev {
     uint8_t *al = nullptr;
     uint64_t *al_off = nullptr;
     uint32_t *al_first = nullptr;
+    uint64_t *key = nullptr;  // k-mer mode: the costs table
+    float *cost = nullptr;
     uint8_t *arena = nullptr;
     uint64_t arena_bytes = 0;
     int sms = 0;
 };
 
 uint64_t align_up(uint64_t b) { return (b + 255) / 256 * 256; }
+
+// the launches and downloads of a k-mer chunk (ra_run_chunk after its uploads): float distances, no status
+int ka_launch(RaCall &call, const RaChunk &c, RaDev &D, const RaBufs &b, const RaItem *d_items, const RaJob *d_jobs, const uint32_t *d_list,
+              size_t n_list, uint8_t *d_scratch, float *d_dist, int32_t *d_call, int64_t *d_quality, std::string &msg) {
+    const uint32_t ni = c.item1 - c.item0, nj = c.job1 - c.job0;
+    const KaParams p{call.kparams.k, call.kparams.gap, D.key, D.cost, call.kparams.n};
+    RA_CUDA(cudaEventRecord(D.e0, D.s));
+    ka_short_kernel<<<(nj + RA_BLOCK - 1) / RA_BLOCK, RA_BLOCK, 0, D.s>>>(b, d_items, c.item0, d_jobs, nj, p, d_dist);
+    RA_CUDA(cudaGetLastError());
+    ++call.st.kernel_launches;
+    if (n_list) {
+        const uint32_t per_block = RA_BLOCK / 32;
+        const uint32_t grid = (uint32_t)std::min<uint64_t>((n_list + per_block - 1) / per_block, 64ull * D.sms);
+        ka_long_kernel<<<grid, RA_BLOCK, 0, D.s>>>(b, d_items, c.item0, d_jobs, d_list, (uint32_t)n_list, p, d_scratch, d_dist);
+        RA_CUDA(cudaGetLastError());
+        ++call.st.kernel_launches;
+    }
+    if (call.decide) {
+        ka_decide_kernel<<<(ni + RA_BLOCK - 1) / RA_BLOCK, RA_BLOCK, 0, D.s>>>(d_items, ni, c.job0, d_dist, d_call, d_quality);
+        RA_CUDA(cudaGetLastError());
+        ++call.st.kernel_launches;
+    }
+    RA_CUDA(cudaEventRecord(D.e1, D.s));
+    if (call.decide) {
+        RA_CUDA(cudaMemcpyAsync(call.call + c.item0, d_call, ni * 4, cudaMemcpyDeviceToHost, D.s));
+        RA_CUDA(cudaMemcpyAsync(call.quality + c.item0, d_quality, ni * 8, cudaMemcpyDeviceToHost, D.s));
+        call.st.d2h_bytes += ni * 12;
+    } else {
+        RA_CUDA(cudaMemcpyAsync(call.kdist + c.job0, d_dist, nj * 4, cudaMemcpyDeviceToHost, D.s));
+        call.st.d2h_bytes += nj * 4;
+    }
+    RA_CUDA(cudaStreamSynchronize(D.s));
+    float ms = 0;
+    RA_CUDA(cudaEventElapsedTime(&ms, D.e0, D.e1));
+    call.st.device_ms += ms;
+    return WHMEC_OK;
+}
 
 }  // namespace
 
@@ -162,6 +262,14 @@ int ra_run_chunk(int device, RaCall &call, const RaChunk &c, std::string &msg) {
             RA_CUDA(cudaMemcpyAsync(D.al_first, call.host.al_first, (uint64_t)(call.n_variants + 1) * 4, cudaMemcpyHostToDevice, D.s));
             call.st.h2d_bytes += nb + (call.n_alleles + 1) * 8 + (uint64_t)(call.n_variants + 1) * 4;
         }
+        if (call.kmerald && call.kparams.n) {
+            const uint64_t nk = call.kparams.n;
+            RA_CUDA(cudaMalloc(&D.key, nk * 8));
+            RA_CUDA(cudaMalloc(&D.cost, nk * 4));
+            RA_CUDA(cudaMemcpyAsync(D.key, call.kparams.key, nk * 8, cudaMemcpyHostToDevice, D.s));
+            RA_CUDA(cudaMemcpyAsync(D.cost, call.kparams.cost, nk * 4, cudaMemcpyHostToDevice, D.s));
+            call.st.h2d_bytes += nk * 12;
+        }
     }
     if (D.arena_bytes < c.bytes) {
         if (D.arena) RA_CUDA(cudaFree(D.arena));
@@ -197,6 +305,7 @@ int ra_run_chunk(int device, RaCall &call, const RaChunk &c, std::string &msg) {
     RA_CUDA(cudaMemcpyAsync(d_r, call.host.ref + c.r_lo, (uint64_t)(c.r_hi - c.r_lo), cudaMemcpyHostToDevice, D.s));
     call.st.h2d_bytes += ni * sizeof(RaItem) + nj * sizeof(RaJob) + list.size() * 4 + (c.q_hi - c.q_lo) + (uint64_t)(c.r_hi - c.r_lo);
     const RaBufs b{d_q, c.q_lo, d_r, c.r_lo, D.al, D.al_off, D.al_first};
+    if (call.kmerald) return ka_launch(call, c, D, b, d_items, d_jobs, d_list, list.size(), d_scratch, (float *)d_dist, d_call, d_quality, msg);
     RA_CUDA(cudaEventRecord(D.e0, D.s));
     ra_short_kernel<<<(nj + RA_BLOCK - 1) / RA_BLOCK, RA_BLOCK, 0, D.s>>>(b, d_items, c.item0, d_jobs, nj, call.params, d_dist, d_status);
     RA_CUDA(cudaGetLastError());
@@ -240,6 +349,8 @@ void ra_close(RaCall &call) {
     cudaFree(D->al);
     cudaFree(D->al_off);
     cudaFree(D->al_first);
+    cudaFree(D->key);
+    cudaFree(D->cost);
     if (D->e0) cudaEventDestroy(D->e0);
     if (D->e1) cudaEventDestroy(D->e1);
     if (D->s) cudaStreamDestroy(D->s);

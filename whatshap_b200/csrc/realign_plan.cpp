@@ -1,5 +1,5 @@
-// Allele detection by re-alignment (whmec_realign, DESIGN §4.11): the host walk, the chunk plan and the two C entry points.
-// The walk restates whatshap/_variants.pyx:10-81 (_iterate_cigar) and the window steps of ReadSetReader.realign
+// Allele detection by re-alignment (whmec_realign, DESIGN §4.11; k-mer mode, §4.12): the host walk, the chunk plan and the C
+// entry points.  The walk restates whatshap/_variants.pyx:10-81 (_iterate_cigar) and the window steps of ReadSetReader.realign
 // (whatshap/variants.py:599-682, 724-831) for one alignment; the device work of a chunk is ra_run_chunk (realign.cu).
 #include "realign_plan.h"
 
@@ -100,7 +100,12 @@ uint64_t ra_job_need(uint64_t q_len, uint64_t target_len, int affine) {
     return std::min(q_len, target_len) <= RA_SHORT ? RA_NO_SCRATCH : (std::max(q_len, target_len) + 15) / 16 * 16;
 }
 
-bool ra_walk_alignment(const whmec_realign_input &in, uint32_t a, std::vector<RaItem> &items, std::vector<RaJob> &jobs, std::string &err) {
+uint64_t ka_job_need(uint64_t q_len, uint64_t target_len) {
+    return q_len <= KA_SHORT && target_len <= KA_SHORT ? RA_NO_SCRATCH : ka_scratch_bytes(q_len, target_len);
+}
+
+bool ra_walk_alignment(const whmec_realign_input &in, uint32_t a, std::vector<RaItem> &items, std::vector<RaJob> &jobs, std::string &err,
+                       const whmec_kmerald_params *km) {
     const uint64_t c0 = in.cigar_off[a], c1 = in.cigar_off[a + 1];
     if (c1 == c0) return true;  // `if not cigartuples: return`
     const CigarView cg{in.cigar_op + c0, in.cigar_len + c0, (uint32_t)(c1 - c0)};
@@ -118,12 +123,14 @@ bool ra_walk_alignment(const whmec_realign_input &in, uint32_t a, std::vector<Ra
         const int64_t ref_len = (int64_t)allele_len(in, index, 0);
         int64_t lr, lq, rr, rq;
         std::string why;
-        if (!prefix_length(cg, true, i, consumed, in.overhang, lr, lq, why)) return fail(index, why);
-        if (!prefix_length(cg, false, i, consumed, ref_len + in.overhang, rr, rq, why)) return fail(index, why);
+        const int64_t window = km ? km->window : in.overhang;
+        if (!prefix_length(cg, true, i, consumed, window, lr, lq, why)) return fail(index, why);
+        if (!prefix_length(cg, false, i, consumed, ref_len + window, rr, rq, why)) return fail(index, why);
         const int64_t pos = in.position[index];
         if (!(pos - lr >= 0)) return fail(index, "the window starts before the reference (assert variant.position - left_ref_bases >= 0)");
         if (!(pos + rr <= (int64_t)in.reference_len))
             return fail(index, "the window ends after the reference (assert variant.position + right_ref_bases <= len(reference))");
+        if (km && !km->has_alt[index]) return fail(index, "the variant has no alternative_allele (a multiallelic variant: the reference raises AttributeError)");
         RaItem it{};
         int64_t qfirst, qn;
         py_slice(qpos - lq, qpos + rq, qlen, qfirst, qn);
@@ -137,7 +144,12 @@ bool ra_walk_alignment(const whmec_realign_input &in, uint32_t a, std::vector<Ra
         it.alignment = a;
         it.job0 = (uint32_t)jobs.size();
         const uint32_t item = (uint32_t)items.size();
-        for (uint32_t k = 0; k < n_alleles; ++k) {
+        if (km) {  // allele 0 and alternative_allele, which the k-mer call reads as slot 2 * index + 1 (whmec_realign_kmerald)
+            const uint64_t alt_len = km->alt_off[index + 1] - km->alt_off[index];
+            jobs.push_back(RaJob{item, 0, ka_job_need(it.q_len, lr + rr)});
+            jobs.push_back(RaJob{item, 1, ka_job_need(it.q_len, lr + alt_len + (uint64_t)std::max<int64_t>(rr - ref_len, 0))});
+        }
+        for (uint32_t k = 0; k < n_alleles && !km; ++k) {
             if (in.restrict_off) {
                 const int32_t *g0 = in.restrict_allele + in.restrict_off[index], *g1 = in.restrict_allele + in.restrict_off[index + 1];
                 if (std::find(g0, g1, (int32_t)k) == g1) continue;
@@ -187,7 +199,7 @@ bool ra_walk_alignment(const whmec_realign_input &in, uint32_t a, std::vector<Ra
     return true;
 }
 
-void ra_plan(const whmec_realign_input &in, RaPlan &plan) {
+void ra_plan(const whmec_realign_input &in, RaPlan &plan, const whmec_kmerald_params *km) {
     const uint32_t n = in.n_alignments;
     const uint32_t threads = host_threads(32);
     const uint32_t n_tasks = std::max(1u, std::min(n, threads * 8));
@@ -198,7 +210,7 @@ void ra_plan(const whmec_realign_input &in, RaPlan &plan) {
     parallel_tasks(n_tasks, threads, [&](uint32_t t) {
         const uint32_t a0 = (uint32_t)((uint64_t)n * t / n_tasks), a1 = (uint32_t)((uint64_t)n * (t + 1) / n_tasks);
         for (uint32_t a = a0; a < a1; ++a) {
-            if (!ra_walk_alignment(in, a, items[t], jobs[t], errs[t])) return;
+            if (!ra_walk_alignment(in, a, items[t], jobs[t], errs[t], km)) return;
             counts[t].push_back(items[t].size());
         }
     });
@@ -318,14 +330,27 @@ void count_jobs(RaCall &call, uint32_t n_items, const RaJob *jobs) {
 
 using namespace whmec;
 
-extern "C" int whmec_realign(const whmec_realign_input *in, int device, whmec_realign_output *out, whmec_realign_stats *stats, char *err,
-                             size_t errlen) {
-    if (!in || !out || (in->n_alignments && (!in->reference_start || !in->cigar_off || !in->query_off)) ||
-        (in->n_variants && (!in->position || !in->allele_first || !in->allele_off)) || in->overhang < 0 ||
-        (in->affine != 0 && in->affine != 1)) {
-        put_err(err, errlen, "whmec_realign: null or malformed arguments");
-        return WHMEC_ERR_INPUT;
-    }
+namespace {
+
+// The checks of a k-mer mode's parameters (name: the entry point), empty when they pass.
+std::string ka_check(const whmec_kmerald_params *km, uint32_t n_variants, bool alts, const char *name) {
+    if (!km || !km->costs || km->kmer_size < 1 || km->kmer_size > 15 || km->window < 0 ||
+        (alts && n_variants && (!km->alt_off || !km->has_alt)))
+        return std::string(name) + ": null or malformed k-mer parameters (kmer_size 1..15, window >= 0)";
+    const whmec_kmer_costs &c = *km->costs;
+    if (c.n >= (1ull << 32) || (c.n && (!c.key || !c.cost))) return std::string(name) + ": null or oversized costs table (n < 2^32)";
+    for (uint64_t i = 1; i < c.n; ++i)
+        if (c.key[i] <= c.key[i - 1]) return std::string(name) + ": the costs' keys are not strictly ascending at entry " + std::to_string(i);
+    return std::string();
+}
+
+KaParams ka_params(const whmec_kmerald_params &km) {
+    return KaParams{(uint32_t)km.kmer_size, km.gap_penalty, km.costs->key, km.costs->cost, (uint32_t)km.costs->n};
+}
+
+// whmec_realign (km == NULL) and whmec_realign_kmerald, after their argument checks
+int realign_call(const whmec_realign_input *in, const whmec_kmerald_params *km, int device, whmec_realign_output *out,
+                 whmec_realign_stats *stats, char *err, size_t errlen) {
     std::memset(out, 0, sizeof(*out));
     for (uint32_t v = 0; v < in->n_variants; ++v)
         if (in->allele_first[v + 1] <= in->allele_first[v]) {
@@ -341,7 +366,7 @@ extern "C" int whmec_realign(const whmec_realign_input *in, int device, whmec_re
     try {
         const auto t0 = std::chrono::steady_clock::now();
         RaPlan plan;
-        ra_plan(*in, plan);
+        ra_plan(*in, plan, km);
         if (!plan.err.empty()) {
             put_err(err, errlen, plan.err);
             return WHMEC_ERR_INPUT;
@@ -355,6 +380,27 @@ extern "C" int whmec_realign(const whmec_realign_input *in, int device, whmec_re
         call.params = RaParams{in->affine, (float)in->mismatch, in->gap_start, in->gap_extend};
         call.items = plan.items.data();
         call.jobs = plan.jobs.data();
+        // k-mer mode: the device's allele slots are, per variant v, an empty slot 2v and alternative_allele as slot 2v + 1, so
+        // that ra_target reads allele 1 of variant v as alternative_allele
+        std::vector<uint64_t> slot_off;
+        std::vector<uint32_t> slot_first;
+        if (km) {
+            const uint32_t nv = in->n_variants;
+            slot_off.resize(2 * (uint64_t)nv + 1);
+            slot_first.resize((uint64_t)nv + 1);
+            slot_off[0] = 0;
+            for (uint32_t v = 0; v < nv; ++v) {
+                slot_first[v] = 2 * v;
+                slot_off[2 * v + 1] = km->alt_off[v];
+                slot_off[2 * v + 2] = km->alt_off[v + 1];
+            }
+            slot_first[nv] = 2 * nv;
+            if (nv) slot_off[0] = km->alt_off[0];
+            call.host = RaBufs{in->query, 0, in->reference, 0, km->alt_bytes, slot_off.data(), slot_first.data()};
+            call.n_alleles = 2 * (uint64_t)nv;
+            call.kmerald = true;
+            call.kparams = ka_params(*km);
+        }
         RawVec<int64_t> dist(nj), quality(ni);
         RawVec<int32_t> called(ni);
         std::vector<uint8_t> status(nj, 0);
@@ -363,7 +409,8 @@ extern "C" int whmec_realign(const whmec_realign_input *in, int device, whmec_re
         call.st.cells = plan.cells;
         call.st.plan_ms = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count();
         const uint64_t fixed = 3 * RA_ALIGN + (call.n_alleles + 1) * 8 + (uint64_t)(in->n_variants + 1) * 4 +
-                               (call.n_alleles ? in->allele_off[call.n_alleles] : 0);
+                               (call.n_alleles ? call.host.al_off[call.n_alleles] : 0) +
+                               (km ? 2 * RA_ALIGN + (uint64_t)call.kparams.n * 12 : 0);
         int rc = ni ? run_chunks(device, call, ni, plan.jobs.data(), budget, fixed, msg) : WHMEC_OK;
         if (rc != WHMEC_OK) {
             put_err(err, errlen, msg);
@@ -403,6 +450,34 @@ extern "C" int whmec_realign(const whmec_realign_input *in, int device, whmec_re
         put_err(err, errlen, "whmec_realign: out of host memory");
         return WHMEC_ERR_UNSUPPORTED;
     }
+}
+
+}  // namespace
+
+extern "C" int whmec_realign(const whmec_realign_input *in, int device, whmec_realign_output *out, whmec_realign_stats *stats, char *err,
+                             size_t errlen) {
+    if (!in || !out || (in->n_alignments && (!in->reference_start || !in->cigar_off || !in->query_off)) ||
+        (in->n_variants && (!in->position || !in->allele_first || !in->allele_off)) || in->overhang < 0 ||
+        (in->affine != 0 && in->affine != 1)) {
+        put_err(err, errlen, "whmec_realign: null or malformed arguments");
+        return WHMEC_ERR_INPUT;
+    }
+    return realign_call(in, nullptr, device, out, stats, err, errlen);
+}
+
+extern "C" int whmec_realign_kmerald(const whmec_realign_input *in, const whmec_kmerald_params *params, int device, whmec_realign_output *out,
+                                     whmec_realign_stats *stats, char *err, size_t errlen) {
+    if (!in || !out || (in->n_alignments && (!in->reference_start || !in->cigar_off || !in->query_off)) ||
+        (in->n_variants && (!in->position || !in->allele_first || !in->allele_off))) {
+        put_err(err, errlen, "whmec_realign_kmerald: null or malformed arguments");
+        return WHMEC_ERR_INPUT;
+    }
+    const std::string bad = ka_check(params, in->n_variants, true, "whmec_realign_kmerald");
+    if (!bad.empty()) {
+        put_err(err, errlen, bad);
+        return WHMEC_ERR_INPUT;
+    }
+    return realign_call(in, params, device, out, stats, err, errlen);
 }
 
 extern "C" void whmec_realign_release(whmec_realign_output *out) {
@@ -475,6 +550,63 @@ extern "C" int whmec_edit_distance_batch(uint32_t n, const uint64_t *query_off, 
         return WHMEC_OK;
     } catch (const std::bad_alloc &) {
         put_err(err, errlen, "whmec_edit_distance_batch: out of host memory");
+        return WHMEC_ERR_UNSUPPORTED;
+    }
+}
+
+extern "C" int whmec_kmer_align_batch(uint32_t n, const uint64_t *s1_off, const uint8_t *s1, const uint64_t *s2_off, const uint8_t *s2,
+                                      const whmec_kmerald_params *params, float *out, int device, whmec_realign_stats *stats, char *err,
+                                      size_t errlen) {
+    if (n && (!s1_off || !s2_off || !out)) {
+        put_err(err, errlen, "whmec_kmer_align_batch: null arguments");
+        return WHMEC_ERR_INPUT;
+    }
+    const std::string bad = ka_check(params, 0, false, "whmec_kmer_align_batch");
+    if (!bad.empty()) {
+        put_err(err, errlen, bad);
+        return WHMEC_ERR_INPUT;
+    }
+    std::string msg;
+    const uint64_t budget = ra_budget(device, msg);
+    if (!msg.empty()) {
+        put_err(err, errlen, msg);
+        return WHMEC_ERR_CUDA;
+    }
+    try {
+        StagedVec<RaItem> items(n);
+        StagedVec<RaJob> jobs(n);
+        uint64_t cells = 0;
+        for (uint32_t i = 0; i < n; ++i) {
+            // a pair is an item whose query is s2 (the columns) and whose allele 0 ("reference" window) is s1 (the rows)
+            const uint64_t l1 = s1_off[i + 1] - s1_off[i], l2 = s2_off[i + 1] - s2_off[i];
+            if (l1 >= (1ull << 31) || l2 >= (1ull << 31)) {
+                put_err(err, errlen, "whmec_kmer_align_batch: pair " + std::to_string(i) + " is longer than 2^31 - 1");
+                return WHMEC_ERR_INPUT;
+            }
+            items[i] = RaItem{s2_off[i], (int64_t)s1_off[i], (uint32_t)l2, (uint32_t)l1, 0, 0, 0, i, 1, i};
+            jobs[i] = RaJob{i, 0, ka_job_need(l2, l1)};
+            cells += l1 * l2;
+        }
+        RaCall call;
+        call.host = RaBufs{s2, 0, s1, 0, nullptr, nullptr, nullptr};
+        call.decide = false;
+        call.kmerald = true;
+        call.kparams = ka_params(*params);
+        call.items = items.data();
+        call.jobs = jobs.data();
+        std::vector<uint8_t> status(n, 0);
+        call.kdist = out, call.status = status.data();
+        count_jobs(call, n, jobs.data());
+        call.st.cells = cells;
+        const int rc = n ? run_chunks(device, call, n, jobs.data(), budget, 2 * RA_ALIGN + (uint64_t)call.kparams.n * 12, msg) : WHMEC_OK;
+        if (rc != WHMEC_OK) {
+            put_err(err, errlen, msg);
+            return rc;
+        }
+        if (stats) *stats = call.st;
+        return WHMEC_OK;
+    } catch (const std::bad_alloc &) {
+        put_err(err, errlen, "whmec_kmer_align_batch: out of host memory");
         return WHMEC_ERR_UNSUPPORTED;
     }
 }

@@ -1,11 +1,13 @@
-// Allele detection by re-alignment (whmec_realign, DESIGN §4.11): the host plan.  realign_plan.cpp walks the CIGARs into items
-// and jobs and cuts them into chunks; realign.cu (and the test-only emulation tests/emul/emul_realign.cpp) runs a chunk.
+// Allele detection by re-alignment (whmec_realign, DESIGN §4.11; k-mer mode whmec_realign_kmerald, §4.12): the host plan.
+// realign_plan.cpp walks the CIGARs into items and jobs and cuts them into chunks; realign.cu (and the test-only emulation
+// tests/emul/emul_realign.cpp) runs a chunk.
 #pragma once
 #include <string>
 #include <vector>
 
 #include "../../include/whmec.h"
 #include "hostpool.h"
+#include "kmerald.h"
 #include "realign.h"
 
 namespace whmec {
@@ -21,14 +23,19 @@ struct RaPlan {
 };
 
 // The walk of one alignment (_iterate_cigar + realign's window and allele steps) appended to `items` and `jobs` (jobs' item
-// fields count from items.size() on entry).  Returns false with the reference's failure in `err`.
-bool ra_walk_alignment(const whmec_realign_input &in, uint32_t a, std::vector<RaItem> &items, std::vector<RaJob> &jobs, std::string &err);
+// fields count from items.size() on entry).  Returns false with the reference's failure in `err`.  With `km` (k-mer mode) the
+// window is km->window instead of the overhang, the jobs are allele 0 and the variant's alternative_allele (allele 1, always;
+// the restricted genotypes are ignored), and a variant without alternative_allele fails.
+bool ra_walk_alignment(const whmec_realign_input &in, uint32_t a, std::vector<RaItem> &items, std::vector<RaJob> &jobs, std::string &err,
+                       const whmec_kmerald_params *km = nullptr);
 // All alignments on the host workers.
-void ra_plan(const whmec_realign_input &in, RaPlan &plan);
+void ra_plan(const whmec_realign_input &in, RaPlan &plan, const whmec_kmerald_params *km = nullptr);
 
 // A job's scratch field as the walk leaves it: RA_NO_SCRATCH for a one-thread job, else the bytes of its warp's work area
 // (unit cost: one byte per text column for the hand-over between 32-word groups; affine: three float rows over the query).
 uint64_t ra_job_need(uint64_t q_len, uint64_t target_len, int affine);
+// The same for a k-mer job: RA_NO_SCRATCH when both strings have at most KA_SHORT bytes, else ka_scratch_bytes.
+uint64_t ka_job_need(uint64_t q_len, uint64_t target_len);
 
 struct RaChunk {
     uint32_t item0 = 0, item1 = 0;  // items [item0, item1) and their jobs [job0, job1)
@@ -52,10 +59,13 @@ struct RaCall {
     uint32_t n_variants = 0;
     uint64_t ref_len = 0;
     RaParams params{};
-    bool decide = true;             // false: distances only (whmec_edit_distance_batch)
+    bool decide = true;             // false: distances only (whmec_edit_distance_batch, whmec_kmer_align_batch)
+    bool kmerald = false;           // k-mer mode: kparams, float distances in kdist
+    KaParams kparams{};             // the caller's costs table (host pointers)
+    float *kdist = nullptr;         // [jobs], k-mer mode without decide
     const RaItem *items = nullptr;
     const RaJob *jobs = nullptr;
-    int64_t *dist = nullptr;        // [jobs]
+    int64_t *dist = nullptr;        // [jobs], unit and affine mode without decide
     uint8_t *status = nullptr;      // [jobs]: 1 = distance beyond int64
     int32_t *call = nullptr;        // [items]: position of the called allele among the item's jobs, -1: none
     int64_t *quality = nullptr;     // [items]

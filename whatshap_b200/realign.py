@@ -7,20 +7,28 @@ against the variant list, the device aligns each covered variant's query window 
 (`whmec_realign`, DESIGN §4.11).  `edit_distances` and `edit_distances_affine_gap` are `whatshap.align.edit_distance` and
 `edit_distance_affine_gap` (with one mismatch cost for every query position) over many pairs.
 
-Where the reference raises (an unknown CIGAR operation, a failed window assert, a restricted genotype that leaves no allele),
-the call raises ValueError naming the first such alignment and variant.  Inputs the reference would only reject later are
-rejected up front: affine mode without its three costs, a negative overhang, a CIGAR without a query sequence, fewer
-restricted genotypes than variants.  kmer alignment (`--use-kmerald`) is not covered.
+With `use_kmerald=True` (`whatshap genotype --use-kmerald`), `detect_alleles` is detect_alleles_by_alignment(...,
+use_kmerald=True, kmerald_costs, kmer_size, kmerald_gappenalty, kmerald_window): each query window (kmerald_window for the
+overhang) and the padded reference and alternative alleles are cut into k-mers (`enumerate_all_kmers`) and aligned with
+`kmer_align` in float32 on the device (`whmec_realign_kmerald`, DESIGN §4.12); the costs are a `KmerCosts` table, packed once
+and reusable across calls.  `kmer_distances` is `kmer_align` over many pairs of strings.
+
+Where the reference raises (an unknown CIGAR operation, a failed window assert, a restricted genotype that leaves no allele,
+in k-mer mode a covered multiallelic variant, which has no `alternative_allele`), the call raises ValueError naming the first
+such alignment and variant.  Inputs the reference would only reject later are rejected up front: affine mode without its three
+costs, a negative overhang or window, a CIGAR without a query sequence, fewer restricted genotypes than variants, k-mer mode
+without costs, a k-mer size outside 1..15.
 """
 from __future__ import annotations
 
+import csv
 import ctypes as C
 from typing import List, Optional, Sequence, Tuple
 
 import numpy as np
 
 from . import _lib
-from ._abi import WHMEC_ERR_INPUT, CRealignInput, CRealignOutput, CRealignStats, raise_for
+from ._abi import WHMEC_ERR_INPUT, CKmeraldParams, CKmerCosts, CRealignInput, CRealignOutput, CRealignStats, raise_for
 
 Call = Tuple[int, int, int]
 
@@ -101,21 +109,116 @@ def pack_input(alignments, variants, reference, restricted_genotypes=None, overh
     return ci, keep
 
 
+_KMER_MAX = 2**30  # k-mers of k <= 15 lie in 1 .. 2^30 - 1
+
+
+def _integral(x):
+    try:
+        i = int(x)
+    except (TypeError, ValueError, OverflowError):
+        return None
+    return i if i == x else None
+
+
+class KmerCosts:
+    """The costs of `kmer_align`: {(ref k-mer, read k-mer): cost}, with read k-mer -5 for a ref k-mer's default, packed once
+    into the sorted table the device searches (keys ref << 32 | read, -5 as 0; costs as float32 of float(value)).  One table
+    serves any number of calls.  Keys no k-mer can ever look up are dropped; a value float() rejects raises ValueError."""
+
+    def __init__(self, mapping):
+        keys, values = [], []
+        for key, value in mapping.items():
+            try:
+                v = float(value)
+            except (TypeError, ValueError) as e:
+                raise ValueError(f"kmer costs: the value {value!r} of {key!r} is not a number float() accepts") from e
+            try:
+                a, b = key
+            except (TypeError, ValueError):
+                continue
+            a, b = _integral(a), _integral(b)
+            if a is None or not 1 <= a < _KMER_MAX or b is None:
+                continue
+            if b == -5:
+                b = 0
+            elif not 1 <= b < _KMER_MAX:
+                continue
+            keys.append((a << 32) | b)
+            values.append(v)
+        key = np.array(keys, np.uint64)
+        with np.errstate(over="ignore"):
+            cost = np.array(values, np.float64).astype(np.float32)
+        order = np.argsort(key, kind="stable")
+        self.key, self.cost = np.ascontiguousarray(key[order]), np.ascontiguousarray(cost[order])
+        self._c = CKmerCosts(len(self.key), _ptr(self.key if len(self.key) else None, C.c_uint64),
+                             _ptr(self.cost if len(self.cost) else None, C.c_float))
+
+    @classmethod
+    def read(cls, path) -> "KmerCosts":
+        """The costs file as `_alignments_to_reads` reads it: tab-separated `ref k-mer, read k-mer, cost`, the last of repeated
+        keys kept."""
+        costs = {}
+        with open(path) as f:
+            for line in csv.reader(f, delimiter="\t"):
+                costs[(int(line[0]), int(line[1]))] = line[2]
+        return cls(costs)
+
+    def __len__(self) -> int:
+        return len(self.key)
+
+
+def _kmerald_params(costs, kmer_size, gap_penalty, window, variants=None):
+    """(whmec_kmerald_params, the objects it points into)."""
+    if costs is None:
+        raise ValueError("k-mer realignment needs kmerald_costs")
+    if not isinstance(costs, KmerCosts):
+        costs = KmerCosts(costs)
+    k = int(kmer_size)
+    if not 1 <= k <= 15:
+        raise ValueError("kmer_size must lie in 1..15")
+    if window < 0:
+        raise ValueError("kmerald_window must be >= 0")
+    keep = [costs]
+    alt_off = alt = has = None
+    if variants is not None:
+        alts = [getattr(v, "alternative_allele", None) for v in variants]
+        has = np.array([a is not None for a in alts] or [0], np.uint8)
+        alt_off, alt = _csr([_bytes(a) if a is not None else b"" for a in alts])
+        keep += [alt_off, alt, has]
+    params = CKmeraldParams(k, float(gap_penalty), int(window), C.pointer(costs._c), _ptr(alt_off, C.c_uint64), _ptr(alt, C.c_uint8),
+                            _ptr(has, C.c_uint8))
+    return params, keep
+
+
 def detect_alleles(alignments, variants, reference, *, restricted_genotypes=None, overhang: int = 10, affine: bool = False,
-                   gap_start=None, gap_extend=None, default_mismatch=None, device: int = 0, stats: Optional[dict] = None,
+                   gap_start=None, gap_extend=None, default_mismatch=None, use_kmerald: bool = False, kmerald_costs=None,
+                   kmer_size: int = 7, kmerald_gappenalty=40, kmerald_window=25, device: int = 0, stats: Optional[dict] = None,
                    library: Optional[C.CDLL] = None) -> List[List[Call]]:
     """Per alignment, the (variant index, allele, quality) tuples of detect_alleles_by_alignment, in its order.
 
     alignments: objects with `reference_start`, `cigartuples` and `query_sequence` (a pysam.AlignedSegment qualifies);
-    variants: objects with `position`, `reference_allele` and `get_alt_allele_list()`; reference: the chromosome (str or
-    bytes); restricted_genotypes: None or one object with `as_vector()` per variant.  `stats` (a dict) receives the
-    call's counters: items, jobs, short_jobs / long_jobs (one thread / one warp per allele alignment), chunks, device_ms.
-    `library`: another build of the library with the same entry point (tests)."""
+    variants: objects with `position`, `reference_allele` and `get_alt_allele_list()` (and, for k-mer mode,
+    `alternative_allele`); reference: the chromosome (str or bytes); restricted_genotypes: None or one object with
+    `as_vector()` per variant.  use_kmerald: k-mer realignment with kmerald_costs (a `KmerCosts` or the dict `kmer_align`
+    takes), kmer_size, kmerald_gappenalty and int(kmerald_window); overhang, affine, its costs and the restricted genotypes
+    are then not used.  `stats` (a dict) receives the call's counters: items, jobs, short_jobs / long_jobs (one thread / one
+    warp per allele alignment), chunks, device_ms.  `library`: another build of the library with the same entry point (tests)."""
     L = library or _lib.lib()
-    ci, keep = pack_input(alignments, variants, reference, restricted_genotypes, overhang, affine, gap_start, gap_extend, default_mismatch)
+    if use_kmerald:
+        window = int(kmerald_window)
+        params, kkeep = _kmerald_params(kmerald_costs, kmer_size, kmerald_gappenalty, window, variants)
+        if restricted_genotypes and len(restricted_genotypes) < len(variants):
+            raise ValueError("restricted_genotypes has fewer entries than variants")
+        ci, keep = pack_input(alignments, variants, reference)
+        keep += kkeep
+    else:
+        ci, keep = pack_input(alignments, variants, reference, restricted_genotypes, overhang, affine, gap_start, gap_extend, default_mismatch)
     out, st = CRealignOutput(), CRealignStats()
     err = C.create_string_buffer(1024)
-    rc = L.whmec_realign(C.byref(ci), device, C.byref(out), C.byref(st), err, len(err))
+    if use_kmerald:
+        rc = L.whmec_realign_kmerald(C.byref(ci), C.byref(params), device, C.byref(out), C.byref(st), err, len(err))
+    else:
+        rc = L.whmec_realign(C.byref(ci), device, C.byref(out), C.byref(st), err, len(err))
     if rc == WHMEC_ERR_INPUT:
         raise ValueError(err.value.decode())
     raise_for(rc, err.value.decode())
@@ -172,3 +275,28 @@ def edit_distances_affine_gap(queries, targets, mismatch, gap_start: int = 1, ga
     """int(edit_distance_affine_gap(queries[i], targets[i], [mismatch] * len(queries[i]), gap_start, gap_extend)) for every i
     (align.pyx:114-196): the float32 Gotoh recurrence, mismatch as a float32, gap costs as C ints (10.9 -> 10)."""
     return _pairs(queries, targets, mismatch, int(gap_start), int(gap_extend), True, device, stats, library)
+
+
+def kmer_distances(seqs1, seqs2, costs, gap_penalty=40, kmer_size: int = 7, *, device: int = 0, stats: Optional[dict] = None,
+                   library: Optional[C.CDLL] = None) -> np.ndarray:
+    """kmer_align(enumerate_all_kmers(seqs1[i], kmer_size), enumerate_all_kmers(seqs2[i], kmer_size), costs, gap_penalty) for
+    every i (align.pyx:199-271), as float32; seqs1 are the rows (the reference's alleles), seqs2 the columns (the reads)."""
+    if len(seqs1) != len(seqs2):
+        raise ValueError("seqs1 and seqs2 differ in length")
+    params, keep = _kmerald_params(costs, kmer_size, gap_penalty, 0)
+    L = library or _lib.lib()
+    n = len(seqs1)
+    off1, s1 = _csr([_bytes(s) for s in seqs1])
+    off2, s2 = _csr([_bytes(s) for s in seqs2])
+    res = np.zeros(max(n, 1), np.float32)
+    st = CRealignStats()
+    err = C.create_string_buffer(512)
+    rc = L.whmec_kmer_align_batch(n, _ptr(off1, C.c_uint64), _ptr(s1, C.c_uint8), _ptr(off2, C.c_uint64), _ptr(s2, C.c_uint8), C.byref(params),
+                                  res.ctypes.data_as(C.POINTER(C.c_float)), device, C.byref(st), err, len(err))
+    del keep
+    if rc == WHMEC_ERR_INPUT:
+        raise ValueError(err.value.decode())
+    raise_for(rc, err.value.decode())
+    if stats is not None:
+        stats.update(st.as_dict())
+    return res[:n]
