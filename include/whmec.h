@@ -21,6 +21,7 @@
  *   whmec_realign          <- ReadSetReader.detect_alleles_by_alignment  whatshap/variants.py:599-912 (allele detection
  *                             by re-alignment, the step that builds the ReadSet)
  *   whmec_realign_kmerald  <- the same with use_kmerald=True  whatshap/variants.py:731-794, align.pyx:199-271
+ *   whmec_learn            <- Caller (the k-mer pair counts of `whatshap learn`)  src/caller.cpp, whatshap/core.pyx:651-671
  *
  * Plain pointers and sizes only.  All input pointers are caller-owned host
  * memory, read-only, and need to stay valid only for the duration of the call.
@@ -428,6 +429,63 @@ int whmec_realign_kmerald(const whmec_realign_input *in, const whmec_kmerald_par
 int whmec_kmer_align_batch(uint32_t n, const uint64_t *s1_off, const uint8_t *s1, const uint64_t *s2_off, const uint8_t *s2,
                            const whmec_kmerald_params *params, float *out, int device, whmec_realign_stats *stats, char *err,
                            size_t errlen);
+
+/* ---- K-mer pair counts of `whatshap learn`: the rows the reference's Caller (src/caller.cpp, whatshap/core.pyx:651-671) writes
+ * for the reads run_learn hands it (whatshap/cli/learn.py), for many reads in one call.  A read's k-mer at column c is counted iff
+ * c > its floor T_r = max(k - 1, pos_m + k - 1 over every read m before it); a read with a single k-mer counts it twice.  The
+ * popped columns (k .. L with `final`, else k .. max(k - 1, max pos_r + k - 1), or the given range) pass the variant windows in
+ * order (pop_column); each remaining column that has counts gives one row per read k-mer, rows ascending by column, then by
+ * read k-mer (the reference's order within a column is its unordered_map's).  The host walks every CIGAR (WHMEC_HOST_THREADS
+ * workers) and cuts the columns into chunks under the free HBM less 512 MB (or WHMEC_LEARN_ARENA_BUDGET bytes); the device emits
+ * one key per kept k-mer, sorts and run-length encodes the keys and attaches the reference k-mers. */
+typedef struct whmec_learn_input {
+    const uint8_t *reference;        /* the chromosome's bytes (only A, C, G and T count; N and lower case leave the k-mer as it is) */
+    uint64_t reference_len;          /* L, k <= L < 2^31 */
+    uint32_t n_alignments;           /* in the order of the add_read calls */
+    const int32_t *reference_start;  /* [n_alignments]: alignment.pos */
+    const uint64_t *cigar_off;       /* [n_alignments + 1] into cigar_op / cigar_len */
+    const uint8_t *cigar_op;         /* pysam codes MIDNSHP=X = 0..8 */
+    const int32_t *cigar_len;        /* >= 0 */
+    const uint64_t *query_off;       /* [n_alignments + 1] into query */
+    const uint8_t *query;            /* query_alignment_sequence bytes */
+    uint32_t n_variants;             /* > 0: the whole list all_variants was given, in its order */
+    const int32_t *variant_pos;      /* [n_variants]: VCF position (1-based) */
+    const int32_t *variant_len;      /* [n_variants]: len(REF) */
+    uint32_t first_variant;          /* the variant list's state before the first popped column (its front), < n_variants */
+    int32_t k;                       /* 1..15 */
+    int32_t window;
+    int32_t final;                   /* 1: pop columns k..L (final_pop); 0: k..max(k - 1, max target) (a Caller that is abandoned) */
+    int64_t col_lo, col_hi;          /* col_lo > 0: pop exactly the columns col_lo..col_hi instead (k <= col_lo, col_hi <= L) */
+    const int32_t *floor;            /* NULL: the floors as above; else [n_alignments]: each read's T_r (>= k - 1) */
+} whmec_learn_input;
+
+typedef struct whmec_learn_output {  /* filled by the library (rows) or by the caller (for whmec_learn_write) */
+    uint64_t n_rows;
+    int32_t *rows;                   /* [n_rows][4]: column, reference k-mer, read k-mer, count */
+    uint32_t next_variant;           /* the variant list's front after the last popped column */
+} whmec_learn_output;
+
+typedef struct whmec_learn_stats {
+    uint64_t alignments;
+    uint64_t kmers;                  /* k-mers the reads enumerate */
+    uint64_t kept;                   /* keys counted (above the floor, in the popped columns; a single k-mer twice) */
+    uint64_t distinct;               /* distinct (column, read k-mer) keys */
+    uint64_t rows;                   /* those in output columns */
+    uint64_t h2d_bytes, d2h_bytes;
+    uint32_t chunks, kernel_launches;
+    float device_ms;                 /* device time of the chunks' launches (CUDA events) */
+    float plan_ms;                   /* host walk, floors, variant windows and chunk cut */
+} whmec_learn_stats;
+
+/* Returns WHMEC_OK, WHMEC_ERR_INPUT for malformed arguments and for every input on which the reference aborts or reads out of
+ * bounds (k outside 1..15, L < k, an empty variant list, a read without a k-mer, P, B or an unknown operation of non-zero length
+ * or a CIGAR that ends while query bytes remain, pos + k - 1 > L or a k-mer column beyond L, positions outside int32): err then
+ * names the first such alignment; WHMEC_ERR_CUDA for a device failure.  out is only filled on WHMEC_OK.  stats may be NULL. */
+int whmec_learn(const whmec_learn_input *in, int device, whmec_learn_output *out, whmec_learn_stats *stats, char *err, size_t errlen);
+void whmec_learn_release(whmec_learn_output *out);
+/* Writes out's rows as the reference does ("%d\t%d\t%d\t%d\n"), appending (append != 0) or truncating.  WHMEC_ERR_INPUT when
+ * the file cannot be written. */
+int whmec_learn_write(const char *path, const whmec_learn_output *out, int append, char *err, size_t errlen);
 
 #ifdef __cplusplus
 }

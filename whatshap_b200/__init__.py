@@ -15,6 +15,7 @@ from .core import (  # noqa: F401
     get_max_genotype_alleles,
     get_max_genotype_ploidy,
 )
+from .learn import Caller, count_kmer_pairs, write_counts  # noqa: F401
 from .types import PhasingAlgorithm  # noqa: F401
 from .variant import Variant  # noqa: F401
 
@@ -23,5 +24,5 @@ PhasingAlgorithm.register(PedMecHeuristic)
 
 __all__ = [
     "Genotype", "GenotypeDPTable", "NumericSampleIds", "Pedigree", "PedigreeDPTable", "PedMecHeuristic", "PhredGenotypeLikelihoods", "Read", "ReadSet",
-    "Variant", "PhasingAlgorithm", "compute_genotypes",
+    "Variant", "PhasingAlgorithm", "compute_genotypes", "Caller", "count_kmer_pairs", "write_counts",
 ]

@@ -377,3 +377,56 @@ class CKmeraldParams(C.Structure):
         ("alt_bytes", _u8p),
         ("has_alt", _u8p),
     ]
+
+
+class CLearnInput(C.Structure):
+    """whmec_learn_input: reference, alignments, variant list and state, k, window and the popped columns of one whmec_learn call."""
+    _fields_ = [
+        ("reference", _u8p),
+        ("reference_len", C.c_uint64),
+        ("n_alignments", C.c_uint32),
+        ("reference_start", C.POINTER(C.c_int32)),
+        ("cigar_off", _u64p),
+        ("cigar_op", _u8p),
+        ("cigar_len", C.POINTER(C.c_int32)),
+        ("query_off", _u64p),
+        ("query", _u8p),
+        ("n_variants", C.c_uint32),
+        ("variant_pos", C.POINTER(C.c_int32)),
+        ("variant_len", C.POINTER(C.c_int32)),
+        ("first_variant", C.c_uint32),
+        ("k", C.c_int32),
+        ("window", C.c_int32),
+        ("final", C.c_int32),
+        ("col_lo", C.c_int64),
+        ("col_hi", C.c_int64),
+        ("floor", C.POINTER(C.c_int32)),
+    ]
+
+
+class CLearnOutput(C.Structure):
+    """whmec_learn_output: rows [n_rows][4] (column, reference k-mer, read k-mer, count) and the variant list's next front."""
+    _fields_ = [
+        ("n_rows", C.c_uint64),
+        ("rows", C.POINTER(C.c_int32)),
+        ("next_variant", C.c_uint32),
+    ]
+
+
+class CLearnStats(C.Structure):
+    _fields_ = [
+        ("alignments", C.c_uint64),
+        ("kmers", C.c_uint64),
+        ("kept", C.c_uint64),
+        ("distinct", C.c_uint64),
+        ("rows", C.c_uint64),
+        ("h2d_bytes", C.c_uint64),
+        ("d2h_bytes", C.c_uint64),
+        ("chunks", C.c_uint32),
+        ("kernel_launches", C.c_uint32),
+        ("device_ms", C.c_float),
+        ("plan_ms", C.c_float),
+    ]
+
+    def as_dict(self) -> dict:
+        return {name: getattr(self, name) for name, _ in self._fields_}

@@ -13,7 +13,7 @@ from typing import List, Optional, Sequence, Tuple, Union
 
 import numpy as np
 
-from ._abi import CHeuristicSolution, CKmeraldParams, CProblem, CRealignInput, CRealignOutput, CRealignStats, CSolution, CStats, FlatProblem, FlatSolution, HeuristicSolution, raise_for
+from ._abi import CHeuristicSolution, CKmeraldParams, CLearnInput, CLearnOutput, CLearnStats, CProblem, CRealignInput, CRealignOutput, CRealignStats, CSolution, CStats, FlatProblem, FlatSolution, HeuristicSolution, raise_for
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("WHMEC_LIBRARY") or os.path.join(HERE, "libwhmec.so")  # WHMEC_LIBRARY: another build of the same library (A/B runs)
@@ -56,6 +56,9 @@ EXPORTS = (
     "whmec_edit_distance_batch",
     "whmec_realign_kmerald",
     "whmec_kmer_align_batch",
+    "whmec_learn",
+    "whmec_learn_release",
+    "whmec_learn_write",
 )
 
 
@@ -130,6 +133,7 @@ def lib() -> C.CDLL:
     L.whmec_genotype_segment_destroy.argtypes = [C.c_void_p]
     L.whmec_genotype_segment_destroy.restype = None
     realign_signatures(L)
+    learn_signatures(L)
     for name in ("whmec_genotype_segment_create", "whmec_genotype_segment_transfer", "whmec_genotype_segment_run"):
         getattr(L, name).restype = C.c_int
     for name in ("whmec_plan_create", "whmec_plan_sweep", "whmec_plan_finish", "whmec_plan_stats", "whmec_solve",
@@ -158,6 +162,17 @@ def realign_signatures(L: C.CDLL) -> C.CDLL:
                                              C.POINTER(CKmeraldParams), C.POINTER(C.c_float), C.c_int, C.POINTER(CRealignStats), C.c_char_p,
                                              C.c_size_t]
         L.whmec_kmer_align_batch.restype = C.c_int
+    return L
+
+
+def learn_signatures(L: C.CDLL) -> C.CDLL:
+    """argtypes of whmec_learn, whmec_learn_release and whmec_learn_write on `L` (this library or a test build)."""
+    L.whmec_learn.argtypes = [C.POINTER(CLearnInput), C.c_int, C.POINTER(CLearnOutput), C.POINTER(CLearnStats), C.c_char_p, C.c_size_t]
+    L.whmec_learn.restype = C.c_int
+    L.whmec_learn_release.argtypes = [C.POINTER(CLearnOutput)]
+    L.whmec_learn_release.restype = None
+    L.whmec_learn_write.argtypes = [C.c_char_p, C.POINTER(CLearnOutput), C.c_int, C.c_char_p, C.c_size_t]
+    L.whmec_learn_write.restype = C.c_int
     return L
 
 
