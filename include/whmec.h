@@ -21,6 +21,8 @@
  *   whmec_realign          <- ReadSetReader.detect_alleles_by_alignment  whatshap/variants.py:599-912 (allele detection
  *                             by re-alignment, the step that builds the ReadSet)
  *   whmec_realign_kmerald  <- the same with use_kmerald=True  whatshap/variants.py:731-794, align.pyx:199-271
+ *   whmec_detect_alleles_cigar <- _detect_alleles (allele detection without a reference)  whatshap/_variants.pyx:84-298,
+ *                             whatshap/variants.py:409-597
  *   whmec_learn            <- Caller (the k-mer pair counts of `whatshap learn`)  src/caller.cpp, whatshap/core.pyx:651-671
  *
  * Plain pointers and sizes only.  All input pointers are caller-owned host
@@ -429,6 +431,30 @@ int whmec_realign_kmerald(const whmec_realign_input *in, const whmec_kmerald_par
 int whmec_kmer_align_batch(uint32_t n, const uint64_t *s1_off, const uint8_t *s1, const uint64_t *s2_off, const uint8_t *s2,
                            const whmec_kmerald_params *params, float *out, int device, whmec_realign_stats *stats, char *err,
                            size_t errlen);
+
+/* ---- Allele detection from the CIGAR alone (`whatshap phase --no-reference`, `whatshap haplotag --no-reference`): per alignment a,
+ * _detect_alleles(normalized, var_progress, 0, a) of ReadSetReader._alignments_to_reads (whatshap/variants.py:409-597,
+ * whatshap/_variants.pyx:84-298), for many alignments in one call.  For alignments in non-decreasing reference_start order (as
+ * _usable_alignments yields them) the reference's running index gives the same answer as first = 0.  The library normalizes the
+ * variants (strip common suffixes, then common prefixes), drops those detect_non_overlapping_variants drops and builds each allele's
+ * match, insert and delete targets; the device walks every CIGAR into enqueued (alignment, variant) items and resolves each item.
+ * The reference, restricted genotypes, overhang and affine fields of whmec_realign_input are ignored; query holds query_sequence. */
+typedef struct whmec_query_qualities {
+    const uint64_t *qual_off;        /* [n_alignments + 1] into qual; an empty range: no (or empty) query_qualities, 30 per base */
+    const uint8_t *qual;             /* query_qualities */
+    const uint8_t *missing;          /* NULL or [n_alignments]: bit 0, query_sequence is None (reading a base raises TypeError);
+                                        bit 1, cigartuples is None (iterating it raises TypeError) */
+} whmec_query_qualities;
+
+/* q may be NULL (30 per base, every sequence and CIGAR present).  Output, release (whmec_realign_release), return codes and the
+ * chunk budget (WHMEC_REALIGN_ARENA_BUDGET) as whmec_realign.  WHMEC_ERR_INPUT for malformed arguments, for positions, lengths and
+ * spans that would leave the reference's C ints, for a variant without alternative alleles that the conflict filter reaches (its
+ * max() raises ValueError), and for every alignment on which the reference raises (an operation outside 0..8: ValueError; a base
+ * or quality index past the end of query_sequence or query_qualities: IndexError; a missing sequence or CIGAR: TypeError); err
+ * then names the first such alignment and the exception.  stats: items = enqueued variants, jobs = short_jobs = their alleles (one
+ * thread per item), long_jobs = long_items = 0, cells = calls, chunks = item windows run. */
+int whmec_detect_alleles_cigar(const whmec_realign_input *in, const whmec_query_qualities *q, int device, whmec_realign_output *out,
+                               whmec_realign_stats *stats, char *err, size_t errlen);
 
 /* ---- K-mer pair counts of `whatshap learn`: the rows the reference's Caller (src/caller.cpp, whatshap/core.pyx:651-671) writes
  * for the reads run_learn hands it (whatshap/cli/learn.py), for many reads in one call.  A read's k-mer at column c is counted iff

@@ -357,6 +357,15 @@ class CRealignStats(C.Structure):
         return {name: getattr(self, name) for name, _ in self._fields_}
 
 
+class CQueryQualities(C.Structure):
+    """whmec_query_qualities: per alignment (CSR) its query_qualities, and which alignments lack query_sequence or cigartuples."""
+    _fields_ = [
+        ("qual_off", _u64p),
+        ("qual", _u8p),
+        ("missing", _u8p),
+    ]
+
+
 class CKmerCosts(C.Structure):
     """whmec_kmer_costs: the sorted costs table of k-mer realignment, keys (ref k-mer << 32 | read k-mer, 0 for -5)."""
     _fields_ = [

@@ -13,7 +13,7 @@ from typing import List, Optional, Sequence, Tuple, Union
 
 import numpy as np
 
-from ._abi import CHeuristicSolution, CKmeraldParams, CLearnInput, CLearnOutput, CLearnStats, CProblem, CRealignInput, CRealignOutput, CRealignStats, CSolution, CStats, FlatProblem, FlatSolution, HeuristicSolution, raise_for
+from ._abi import CHeuristicSolution, CKmeraldParams, CLearnInput, CLearnOutput, CLearnStats, CProblem, CQueryQualities, CRealignInput, CRealignOutput, CRealignStats, CSolution, CStats, FlatProblem, FlatSolution, HeuristicSolution, raise_for
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("WHMEC_LIBRARY") or os.path.join(HERE, "libwhmec.so")  # WHMEC_LIBRARY: another build of the same library (A/B runs)
@@ -56,6 +56,7 @@ EXPORTS = (
     "whmec_edit_distance_batch",
     "whmec_realign_kmerald",
     "whmec_kmer_align_batch",
+    "whmec_detect_alleles_cigar",
     "whmec_learn",
     "whmec_learn_release",
     "whmec_learn_write",
@@ -133,6 +134,7 @@ def lib() -> C.CDLL:
     L.whmec_genotype_segment_destroy.argtypes = [C.c_void_p]
     L.whmec_genotype_segment_destroy.restype = None
     realign_signatures(L)
+    cigar_alleles_signatures(L)
     learn_signatures(L)
     for name in ("whmec_genotype_segment_create", "whmec_genotype_segment_transfer", "whmec_genotype_segment_run"):
         getattr(L, name).restype = C.c_int
@@ -140,6 +142,16 @@ def lib() -> C.CDLL:
                  "whmec_segment_create", "whmec_segment_transfer", "whmec_segment_sweep", "whmec_segment_exits",
                  "whmec_segment_finish"):
         getattr(L, name).restype = C.c_int
+    return L
+
+
+def cigar_alleles_signatures(L: C.CDLL) -> C.CDLL:
+    """argtypes of whmec_detect_alleles_cigar and whmec_realign_release on `L` (this library or a test build that exports them)."""
+    L.whmec_detect_alleles_cigar.argtypes = [C.POINTER(CRealignInput), C.POINTER(CQueryQualities), C.c_int, C.POINTER(CRealignOutput),
+                                             C.POINTER(CRealignStats), C.c_char_p, C.c_size_t]
+    L.whmec_detect_alleles_cigar.restype = C.c_int
+    L.whmec_realign_release.argtypes = [C.POINTER(CRealignOutput)]
+    L.whmec_realign_release.restype = None
     return L
 
 

@@ -13,6 +13,15 @@ overhang) and the padded reference and alternative alleles are cut into k-mers (
 `kmer_align` in float32 on the device (`whmec_realign_kmerald`, DESIGN §4.12); the costs are a `KmerCosts` table, packed once
 and reusable across calls.  `kmer_distances` is `kmer_align` over many pairs of strings.
 
+With `reference=None` (`whatshap phase --no-reference`, `whatshap haplotag --no-reference`), `detect_alleles` is
+_alignments_to_reads without a reference: per alignment, `_detect_alleles(normalized, var_progress, 0, alignment)`
+(whatshap/_variants.pyx:84-298) over the normalized variants that `detect_non_overlapping_variants` keeps, reading the query
+bases and `query_qualities` at the CIGAR's insertions, deletions and matches (`whmec_detect_alleles_cigar`, DESIGN §4.14); the
+re-alignment and k-mer options are not used.  For alignments in non-decreasing `reference_start` order the reference's running
+index gives the same answer as starting at 0.  Where that code raises (an operation outside 0..8, a base or quality index past the
+end of the query, a missing query sequence or CIGAR, a variant without alternatives), the call raises ValueError naming the first
+such alignment (or the variant) and the reference's exception.
+
 Where the reference raises (an unknown CIGAR operation, a failed window assert, a restricted genotype that leaves no allele,
 in k-mer mode a covered multiallelic variant, which has no `alternative_allele`), the call raises ValueError naming the first
 such alignment and variant.  Inputs the reference would only reject later are rejected up front: affine mode without its three
@@ -28,7 +37,7 @@ from typing import List, Optional, Sequence, Tuple
 import numpy as np
 
 from . import _lib
-from ._abi import WHMEC_ERR_INPUT, CKmeraldParams, CKmerCosts, CRealignInput, CRealignOutput, CRealignStats, raise_for
+from ._abi import WHMEC_ERR_INPUT, CKmeraldParams, CKmerCosts, CQueryQualities, CRealignInput, CRealignOutput, CRealignStats, raise_for
 
 Call = Tuple[int, int, int]
 
@@ -107,6 +116,79 @@ def pack_input(alignments, variants, reference, restricted_genotypes=None, overh
         _ptr(ref, C.c_uint8), len(reference), int(overhang), int(bool(affine)),
         int(gap_start) if affine else 0, int(gap_extend) if affine else 0, float(default_mismatch) if affine else 0.0)
     return ci, keep
+
+
+def pack_cigar_input(alignments, variants):
+    """(whmec_realign_input, whmec_query_qualities, the arrays they point into) of one detect_alleles call without a reference."""
+    n = len(alignments)
+    cigars, queries, quals = [], [], []
+    missing = np.zeros(max(n, 1), np.uint8)
+    for k, a in enumerate(alignments):
+        cg, seq, qq = a.cigartuples, a.query_sequence, getattr(a, "query_qualities", None)
+        missing[k] = (seq is None) | (cg is None) << 1
+        cigars.append(cg or ())
+        queries.append(_bytes(seq) if seq is not None else b"")
+        quals.append(bytes(qq) if qq is not None and len(qq) else b"")
+    starts = _int32([a.reference_start for a in alignments], "reference_start")
+    cigar_off = np.zeros(n + 1, np.uint64)
+    if n:
+        np.cumsum(np.fromiter(map(len, cigars), np.uint64, n), out=cigar_off[1:])
+    flat = np.array([x for cg in cigars for x in cg], dtype=np.int64).reshape(-1, 2)
+    ops = flat[:, 0]
+    cigar_op = np.where((ops >= 0) & (ops <= 254), ops, 255).astype(np.uint8)
+    cigar_len = _int32(flat[:, 1], "CIGAR length")
+    query_off, query = _csr(queries)
+    qual_off, qual = _csr(quals)
+    positions = _int32([v.position for v in variants], "variant position")
+    alleles, first = [], [0]
+    for v in variants:
+        alleles.append(_bytes(v.reference_allele))
+        alleles.extend(_bytes(x) for x in v.get_alt_allele_list())
+        first.append(len(alleles))
+    allele_first = np.array(first, np.uint32)
+    allele_off, allele_bytes = _csr(alleles)
+    keep = [starts, cigar_off, cigar_op, cigar_len, query_off, query, qual_off, qual, missing, positions, allele_first, allele_off, allele_bytes]
+    none8 = C.cast(None, C.POINTER(C.c_uint8))
+    ci = CRealignInput(
+        n, _ptr(starts, C.c_int32), _ptr(cigar_off, C.c_uint64), _ptr(cigar_op, C.c_uint8), _ptr(cigar_len, C.c_int32),
+        _ptr(query_off, C.c_uint64), _ptr(query, C.c_uint8), len(variants), _ptr(positions, C.c_int32), _ptr(allele_first, C.c_uint32),
+        _ptr(allele_off, C.c_uint64), _ptr(allele_bytes, C.c_uint8), C.cast(None, C.POINTER(C.c_uint64)), C.cast(None, C.POINTER(C.c_int32)),
+        none8, 0, 0, 0, 0, 0, 0.0)
+    cq = CQueryQualities(_ptr(qual_off, C.c_uint64), _ptr(qual, C.c_uint8), _ptr(missing, C.c_uint8))
+    return ci, cq, keep
+
+
+def _calls(L, out, n):
+    """The per-alignment call lists of a filled whmec_realign_output, which is released."""
+    try:
+        off = np.ctypeslib.as_array(out.call_off, (n + 1,)).copy()
+        total = int(off[-1])
+        if total:
+            var = np.ctypeslib.as_array(out.variant, (total,)).tolist()
+            al = np.ctypeslib.as_array(out.allele, (total,)).tolist()
+            ql = np.ctypeslib.as_array(out.quality, (total,)).tolist()
+        else:
+            var = al = ql = []
+    finally:
+        L.whmec_realign_release(C.byref(out))
+    calls = list(zip(var, al, ql))
+    return [calls[off[k]:off[k + 1]] for k in range(n)]
+
+
+def _detect_alleles_cigar(alignments, variants, device, stats, library):
+    L = library or _lib.lib()
+    ci, cq, keep = pack_cigar_input(alignments, variants)
+    out, st = CRealignOutput(), CRealignStats()
+    err = C.create_string_buffer(1024)
+    rc = L.whmec_detect_alleles_cigar(C.byref(ci), C.byref(cq), device, C.byref(out), C.byref(st), err, len(err))
+    del keep
+    if rc == WHMEC_ERR_INPUT:
+        raise ValueError(err.value.decode())
+    raise_for(rc, err.value.decode())
+    calls = _calls(L, out, len(alignments))
+    if stats is not None:
+        stats.update(st.as_dict())
+    return calls
 
 
 _KMER_MAX = 2**30  # k-mers of k <= 15 lie in 1 .. 2^30 - 1
@@ -201,8 +283,11 @@ def detect_alleles(alignments, variants, reference, *, restricted_genotypes=None
     `alternative_allele`); reference: the chromosome (str or bytes); restricted_genotypes: None or one object with
     `as_vector()` per variant.  use_kmerald: k-mer realignment with kmerald_costs (a `KmerCosts` or the dict `kmer_align`
     takes), kmer_size, kmerald_gappenalty and int(kmerald_window); overhang, affine, its costs and the restricted genotypes
-    are then not used.  `stats` (a dict) receives the call's counters: items, jobs, short_jobs / long_jobs (one thread / one
+    are then not used.  reference=None: detection from the CIGAR alone (`--no-reference`), reading `query_qualities` where the
+    alignment has it; every re-alignment and k-mer option is then not used.  `stats` (a dict) receives the call's counters: items, jobs, short_jobs / long_jobs (one thread / one
     warp per allele alignment), chunks, device_ms.  `library`: another build of the library with the same entry point (tests)."""
+    if reference is None:
+        return _detect_alleles_cigar(alignments, variants, device, stats, library)
     L = library or _lib.lib()
     if use_kmerald:
         window = int(kmerald_window)
@@ -222,23 +307,11 @@ def detect_alleles(alignments, variants, reference, *, restricted_genotypes=None
     if rc == WHMEC_ERR_INPUT:
         raise ValueError(err.value.decode())
     raise_for(rc, err.value.decode())
-    try:
-        n = len(alignments)
-        off = np.ctypeslib.as_array(out.call_off, (n + 1,)).copy()
-        total = int(off[-1])
-        if total:
-            var = np.ctypeslib.as_array(out.variant, (total,)).tolist()
-            al = np.ctypeslib.as_array(out.allele, (total,)).tolist()
-            ql = np.ctypeslib.as_array(out.quality, (total,)).tolist()
-        else:
-            var = al = ql = []
-    finally:
-        L.whmec_realign_release(C.byref(out))
+    calls = _calls(L, out, len(alignments))
     del keep
     if stats is not None:
         stats.update(st.as_dict())
-    calls = list(zip(var, al, ql))
-    return [calls[off[k]:off[k + 1]] for k in range(n)]
+    return calls
 
 
 def _pairs(queries, targets, mismatch, gap_start, gap_extend, affine, device, stats, library):
