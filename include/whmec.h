@@ -24,6 +24,7 @@
  *   whmec_detect_alleles_cigar <- _detect_alleles (allele detection without a reference)  whatshap/_variants.pyx:84-298,
  *                             whatshap/variants.py:409-597
  *   whmec_learn            <- Caller (the k-mer pair counts of `whatshap learn`)  src/caller.cpp, whatshap/core.pyx:651-671
+ *   whmec_haplotag         <- prepare_haplotag_information (read assignment of `whatshap haplotag`)  whatshap/cli/haplotag.py:322-427
  *
  * Plain pointers and sizes only.  All input pointers are caller-owned host
  * memory, read-only, and need to stay valid only for the duration of the call.
@@ -512,6 +513,64 @@ void whmec_learn_release(whmec_learn_output *out);
 /* Writes out's rows as the reference does ("%d\t%d\t%d\t%d\n"), appending (append != 0) or truncating.  WHMEC_ERR_INPUT when
  * the file cannot be written. */
 int whmec_learn_write(const char *path, const whmec_learn_output *out, int append, char *err, size_t errlen);
+
+/* ---- Read assignment of `whatshap haplotag`: the sums of prepare_haplotag_information (whatshap/cli/haplotag.py), for the
+ * reads of many samples in one call.  Per sample, in read order, a read whose representation is already processed is skipped;
+ * otherwise it opens a group with the unprocessed reads of its BX id within linked_read_cutoff of its reference_start (in read
+ * order), and every member's representation becomes processed.  The group's entries (opening read first, then the linked
+ * reads, each in its own order) add their quality to (block, h) for every phase-tuple index h whose allele equals theirs.  The
+ * group takes the block with the highest maximum score (ties: the block matched first), in it the haplotype with the highest
+ * score (ties: the lowest index; haplotypes no allele matched score 0), and quality = best - second best of the ploidy scores.
+ * The host walks the groups and cuts them into chunks under the free HBM less 512 MB (or WHMEC_HAPLOTAG_ARENA_BUDGET bytes); the
+ * device emits one (group, block, haplotype) key per match, radix-sorts the keys and reduces each group's runs. */
+typedef struct whmec_haplotag_input {
+    uint32_t n_samples;
+    const uint64_t *phase_off;       /* [n_samples + 1] into phase_pos / phase_block / allele_off */
+    const int64_t *phase_pos;        /* per sample ascending, distinct: the positions with a phase and a block id */
+    const int64_t *phase_block;      /* int(block_id) */
+    const uint64_t *allele_off;      /* [phase_off[n_samples] + 1] into allele */
+    const int32_t *allele;           /* the phase tuples (an allele outside int32 or None as -1) */
+    uint32_t n_reads;                /* every sample's reads, samples in ascending order, each sample's in ReadSet order */
+    const uint64_t *read_off;        /* [n_reads + 1] into the entries */
+    const int64_t *entry_pos;
+    const int32_t *entry_allele;     /* an allele outside int32 as -1 */
+    const int32_t *entry_quality;
+    const uint32_t *read_sample;     /* [n_reads] < n_samples, non-decreasing */
+    const int64_t *read_repr;        /* [n_reads] interned representation, >= 0 */
+    const int64_t *read_bx;          /* [n_reads] interned BX tag, -1 for none (or when linked reads are ignored) */
+    const int64_t *reference_start;  /* [n_reads] */
+    int64_t ploidy;
+    int64_t linked_read_cutoff;
+} whmec_haplotag_input;
+
+typedef struct whmec_haplotag_output {  /* caller-allocated [n_reads] arrays */
+    int64_t *group;                  /* the group's opening read, -1 for a skipped read */
+    int32_t *n_blocks;               /* at an opening read: blocks its group matched (0 elsewhere) */
+    int64_t *block;                  /* at an opening read: the chosen block id */
+    int32_t *haplotype;              /* at an opening read: the haplotype, -1 when not tagged (no block, or quality 0) */
+    int64_t *quality;                /* at an opening read: best - second best score */
+    int32_t error_kind;              /* the first error in visit order: 0 none, 1 AssertionError (allele not 0 or 1), 2 KeyError
+                                        (position without phase), 3 IndexError (a match at h >= ploidy, or ploidy < 2 at a choice) */
+    int64_t error_read;              /* the read it happened at (the opening read for a choice) */
+    int64_t error_entry;             /* the entry of that read, -1 for a choice */
+} whmec_haplotag_output;
+
+typedef struct whmec_haplotag_stats {
+    uint64_t entries;                /* entries of the groups */
+    uint64_t groups;
+    uint64_t keys;                   /* matches (one key each) */
+    uint64_t runs;                   /* distinct (group, block, haplotype) */
+    uint64_t h2d_bytes, d2h_bytes;
+    uint32_t chunks, kernel_launches;
+    float device_ms;                 /* device time of the chunks' launches (CUDA events) */
+    float plan_ms;                   /* host group walk and chunk cut */
+} whmec_haplotag_stats;
+
+/* Returns WHMEC_OK (also when error_kind is set: then only the error fields are meaningful), WHMEC_ERR_INPUT for malformed
+ * arguments, WHMEC_ERR_UNSUPPORTED when one group's keys cannot be sorted in one call (more than 2^30 matches, or more than 64
+ * key bits), WHMEC_ERR_CUDA for a device failure.  stats may be NULL. */
+int whmec_haplotag(const whmec_haplotag_input *in, int device, whmec_haplotag_output *out, whmec_haplotag_stats *stats, char *err,
+                   size_t errlen);
 
 #ifdef __cplusplus
 }

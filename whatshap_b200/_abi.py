@@ -439,3 +439,58 @@ class CLearnStats(C.Structure):
 
     def as_dict(self) -> dict:
         return {name: getattr(self, name) for name, _ in self._fields_}
+
+
+class CHaplotagInput(C.Structure):
+    """whmec_haplotag_input: every sample's phase table and reads (entries as CSR) of one whmec_haplotag call."""
+    _fields_ = [
+        ("n_samples", C.c_uint32),
+        ("phase_off", _u64p),
+        ("phase_pos", C.POINTER(C.c_int64)),
+        ("phase_block", C.POINTER(C.c_int64)),
+        ("allele_off", _u64p),
+        ("allele", C.POINTER(C.c_int32)),
+        ("n_reads", C.c_uint32),
+        ("read_off", _u64p),
+        ("entry_pos", C.POINTER(C.c_int64)),
+        ("entry_allele", C.POINTER(C.c_int32)),
+        ("entry_quality", C.POINTER(C.c_int32)),
+        ("read_sample", C.POINTER(C.c_uint32)),
+        ("read_repr", C.POINTER(C.c_int64)),
+        ("read_bx", C.POINTER(C.c_int64)),
+        ("reference_start", C.POINTER(C.c_int64)),
+        ("ploidy", C.c_int64),
+        ("linked_read_cutoff", C.c_int64),
+    ]
+
+
+class CHaplotagOutput(C.Structure):
+    """whmec_haplotag_output: caller-allocated [n_reads] arrays and the first error."""
+    _fields_ = [
+        ("group", C.POINTER(C.c_int64)),
+        ("n_blocks", C.POINTER(C.c_int32)),
+        ("block", C.POINTER(C.c_int64)),
+        ("haplotype", C.POINTER(C.c_int32)),
+        ("quality", C.POINTER(C.c_int64)),
+        ("error_kind", C.c_int32),
+        ("error_read", C.c_int64),
+        ("error_entry", C.c_int64),
+    ]
+
+
+class CHaplotagStats(C.Structure):
+    _fields_ = [
+        ("entries", C.c_uint64),
+        ("groups", C.c_uint64),
+        ("keys", C.c_uint64),
+        ("runs", C.c_uint64),
+        ("h2d_bytes", C.c_uint64),
+        ("d2h_bytes", C.c_uint64),
+        ("chunks", C.c_uint32),
+        ("kernel_launches", C.c_uint32),
+        ("device_ms", C.c_float),
+        ("plan_ms", C.c_float),
+    ]
+
+    def as_dict(self) -> dict:
+        return {name: getattr(self, name) for name, _ in self._fields_}

@@ -13,7 +13,7 @@ from typing import List, Optional, Sequence, Tuple, Union
 
 import numpy as np
 
-from ._abi import CHeuristicSolution, CKmeraldParams, CLearnInput, CLearnOutput, CLearnStats, CProblem, CQueryQualities, CRealignInput, CRealignOutput, CRealignStats, CSolution, CStats, FlatProblem, FlatSolution, HeuristicSolution, raise_for
+from ._abi import CHaplotagInput, CHaplotagOutput, CHaplotagStats, CHeuristicSolution, CKmeraldParams, CLearnInput, CLearnOutput, CLearnStats, CProblem, CQueryQualities, CRealignInput, CRealignOutput, CRealignStats, CSolution, CStats, FlatProblem, FlatSolution, HeuristicSolution, raise_for
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("WHMEC_LIBRARY") or os.path.join(HERE, "libwhmec.so")  # WHMEC_LIBRARY: another build of the same library (A/B runs)
@@ -60,6 +60,7 @@ EXPORTS = (
     "whmec_learn",
     "whmec_learn_release",
     "whmec_learn_write",
+    "whmec_haplotag",
 )
 
 
@@ -136,6 +137,7 @@ def lib() -> C.CDLL:
     realign_signatures(L)
     cigar_alleles_signatures(L)
     learn_signatures(L)
+    haplotag_signatures(L)
     for name in ("whmec_genotype_segment_create", "whmec_genotype_segment_transfer", "whmec_genotype_segment_run"):
         getattr(L, name).restype = C.c_int
     for name in ("whmec_plan_create", "whmec_plan_sweep", "whmec_plan_finish", "whmec_plan_stats", "whmec_solve",
@@ -185,6 +187,14 @@ def learn_signatures(L: C.CDLL) -> C.CDLL:
     L.whmec_learn_release.restype = None
     L.whmec_learn_write.argtypes = [C.c_char_p, C.POINTER(CLearnOutput), C.c_int, C.c_char_p, C.c_size_t]
     L.whmec_learn_write.restype = C.c_int
+    return L
+
+
+def haplotag_signatures(L: C.CDLL) -> C.CDLL:
+    """argtypes of whmec_haplotag on `L` (this library or a test build)."""
+    L.whmec_haplotag.argtypes = [C.POINTER(CHaplotagInput), C.c_int, C.POINTER(CHaplotagOutput), C.POINTER(CHaplotagStats), C.c_char_p,
+                                 C.c_size_t]
+    L.whmec_haplotag.restype = C.c_int
     return L
 
 

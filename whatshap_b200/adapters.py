@@ -390,3 +390,23 @@ def make_compute_genotypes(core_module):
         return [Genotype(alleles[g]) if g >= 0 else Genotype([]) for g in gt.tolist()], [tuple(row) for row in gl.tolist()]
 
     return compute_genotypes
+
+
+def make_prepare_haplotag_information(haplotag_module):
+    """`prepare_haplotag_information` (whatshap_b200.haplotag) with its keys built from `haplotag_module`'s own
+    ReadAlignmentRepresentation and PrimaryInfo, so that assigning it in place of the reference's function lets an unchanged
+    `run_haplotag` look the reads up (a dataclass compares equal only to instances of its own class):
+
+        import whatshap.cli.haplotag as h, whatshap_b200.adapters as a
+        h.prepare_haplotag_information = a.make_prepare_haplotag_information(h)
+    """
+    from . import haplotag
+
+    repr_cls, info_cls = haplotag_module.ReadAlignmentRepresentation, haplotag_module.PrimaryInfo
+
+    def prepare_haplotag_information(variant_table, shared_samples, phased_input_reader, regions, ignore_linked_read, linked_read_cutoff,
+                                     ploidy, supplementary_strategy=None, *, device=0, stats=None, library=None):
+        return haplotag._prepare(repr_cls, info_cls, variant_table, shared_samples, phased_input_reader, regions, ignore_linked_read,
+                                 linked_read_cutoff, ploidy, device, stats, library)
+
+    return prepare_haplotag_information
