@@ -25,6 +25,7 @@
  *                             whatshap/variants.py:409-597
  *   whmec_learn            <- Caller (the k-mer pair counts of `whatshap learn`)  src/caller.cpp, whatshap/core.pyx:651-671
  *   whmec_haplotag         <- prepare_haplotag_information (read assignment of `whatshap haplotag`)  whatshap/cli/haplotag.py:322-427
+ *   whmec_haplotagphase    <- compute_votes + best_candidate + consensus (`whatshap haplotagphase`)  whatshap/cli/haplotagphase.py:203-395
  *
  * Plain pointers and sizes only.  All input pointers are caller-owned host
  * memory, read-only, and need to stay valid only for the duration of the call.
@@ -571,6 +572,85 @@ typedef struct whmec_haplotag_stats {
  * key bits), WHMEC_ERR_CUDA for a device failure.  stats may be NULL. */
 int whmec_haplotag(const whmec_haplotag_input *in, int device, whmec_haplotag_output *out, whmec_haplotag_stats *stats, char *err,
                    size_t errlen);
+
+/* ---- Votes of `whatshap haplotagphase`: compute_votes, best_candidate and consensus (whatshap/cli/haplotagphase.py) for many
+ * samples in one call.  Per sample, a read with HP_tag < 1 or PS_tag < 1 is skipped, one with HP_tag > 2 is skipped and counted;
+ * every entry of the others at a heterozygous position adds its quality to the key (PS_tag - 1, (HP_tag - 1) ^ allele_to_id
+ * [allele]) of its position, the first read to reach (position, phase set) inserting (ps, 0) and (ps, 1).  A position takes the
+ * key with the highest score (ties: the key inserted first), q = score / total as a double; an unphased position is dropped when
+ * 100 q < gap_threshold or (only_indels and it is an SNV).  Positions come out in the order the reads first reached them.
+ * The runs form (n_runs_pos > 0 in place of reads) hands over votes a caller holds: per position its (ps, h, score) in key
+ * order, chosen by the same rule.  The host bins the entries by position and cuts whole positions of one sample into chunks under
+ * the free HBM less 512 MB (or WHMEC_HAPLOTAGPHASE_ARENA_BUDGET bytes); the device emits one key per entry, radix-sorts the keys,
+ * walks each position's runs in one thread and orders positions and keys by first entry. */
+typedef struct whmec_haplotagphase_input {
+    uint32_t n_samples;
+    const uint64_t *pos_off;         /* [n_samples + 1] into the position arrays */
+    const int64_t *pos;              /* per sample ascending, distinct */
+    const uint8_t *pos_flags;        /* 1 homozygous, 2 phased (phase is not None), 4 SNV */
+    const uint64_t *a2i_off;         /* [pos_off[n_samples] + 1]: allele -> id pairs, merged as the reference merges records */
+    const int64_t *a2i_allele;
+    const int64_t *a2i_id;
+    const uint64_t *i2a_off;         /* [pos_off[n_samples] + 1]: id -> allele pairs */
+    const int64_t *i2a_id;
+    const int64_t *i2a_allele;
+    uint64_t n_reads;                /* the vote form: every sample's reads, samples ascending */
+    const uint32_t *read_sample;     /* [n_reads], non-decreasing */
+    const int64_t *read_hp;          /* HP_tag */
+    const int64_t *read_ps;          /* PS_tag */
+    const uint64_t *read_off;        /* [n_reads + 1] into the entries */
+    const int64_t *entry_pos;
+    const int64_t *entry_allele;
+    const int32_t *entry_quality;
+    uint64_t n_runs_pos;             /* the runs form: voted positions, each a position of its sample's table, in vote order */
+    const uint32_t *runs_sample;     /* [n_runs_pos], non-decreasing */
+    const int64_t *runs_pos;
+    const uint64_t *run_off;         /* [n_runs_pos + 1] into the runs */
+    const int64_t *run_ps;
+    const int64_t *run_h;
+    const int64_t *run_score;
+    double gap_threshold;
+    int32_t only_indels;
+} whmec_haplotagphase_input;
+
+typedef struct whmec_haplotagphase_output {
+    uint64_t *voted_off;             /* caller-allocated [n_samples + 1]: sample s's voted positions in [voted_off[s], voted_off[s+1]) */
+    uint64_t *skipped;               /* caller-allocated [n_samples]: reads with HP_tag > 2 */
+    int32_t *entry_error;            /* caller-allocated [n_samples]: the sample's first vote error, 0 none, 1 KeyError (position
+                                        missing), 2 KeyError (allele missing from allele_to_id), 3 KeyError (ht ^ id not 0 or 1) */
+    uint64_t *entry_error_at;        /* caller-allocated [n_samples]: its entry (an index into entry_pos) */
+    /* library-allocated, [n_voted] per position in vote order, freed by whmec_haplotagphase_release */
+    uint64_t n_voted;
+    int64_t *voted_pos;
+    int64_t *phase_set;              /* the best key's ps (PS_tag - 1, or run_ps) */
+    int64_t *haplotype;              /* the best key's h */
+    int64_t *score;
+    int64_t *total;
+    int64_t *allele;                 /* [n_voted][2]: id_to_allele[h], id_to_allele[1 - h] of a kept position */
+    uint8_t *kept;
+    int32_t *error;                  /* 0, 1 ZeroDivisionError (total 0), 2 KeyError (id_to_allele of a kept position), 3 ValueError
+                                        (|score| or |total| reaches 2^53), 4 IndexError (a runs-form position without runs) */
+    /* the vote form: every position's keys in insertion order, (ps, 0) and (ps, 1) per phase set */
+    uint64_t *key_off;               /* [n_voted + 1] into the keys */
+    int64_t *key_ps;
+    int64_t *key_score;              /* h alternates 0, 1 */
+} whmec_haplotagphase_output;
+
+typedef struct whmec_haplotagphase_stats {
+    uint64_t entries;                /* entries that voted */
+    uint64_t positions;              /* voted positions */
+    uint64_t records;                /* distinct (position, phase set) */
+    uint64_t h2d_bytes, d2h_bytes;
+    uint32_t chunks, kernel_launches;
+    float device_ms;                 /* device time of the chunks' launches (CUDA events) */
+    float plan_ms;                   /* host binning, chunk cut and gather */
+} whmec_haplotagphase_stats;
+
+/* Returns WHMEC_OK (errors of the reference are reported in entry_error and error), WHMEC_ERR_INPUT for malformed arguments,
+ * WHMEC_ERR_UNSUPPORTED when one position has 2^31 entries or more, WHMEC_ERR_CUDA for a device failure.  stats may be NULL. */
+int whmec_haplotagphase(const whmec_haplotagphase_input *in, int device, whmec_haplotagphase_output *out, whmec_haplotagphase_stats *stats,
+                        char *err, size_t errlen);
+void whmec_haplotagphase_release(whmec_haplotagphase_output *out);
 
 #ifdef __cplusplus
 }

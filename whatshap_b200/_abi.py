@@ -494,3 +494,76 @@ class CHaplotagStats(C.Structure):
 
     def as_dict(self) -> dict:
         return {name: getattr(self, name) for name, _ in self._fields_}
+
+
+class CHaplotagphaseInput(C.Structure):
+    """whmec_haplotagphase_input: every sample's positions and allele tables, and its reads (vote form) or runs (runs form)."""
+    _fields_ = [
+        ("n_samples", C.c_uint32),
+        ("pos_off", _u64p),
+        ("pos", C.POINTER(C.c_int64)),
+        ("pos_flags", _u8p),
+        ("a2i_off", _u64p),
+        ("a2i_allele", C.POINTER(C.c_int64)),
+        ("a2i_id", C.POINTER(C.c_int64)),
+        ("i2a_off", _u64p),
+        ("i2a_id", C.POINTER(C.c_int64)),
+        ("i2a_allele", C.POINTER(C.c_int64)),
+        ("n_reads", C.c_uint64),
+        ("read_sample", C.POINTER(C.c_uint32)),
+        ("read_hp", C.POINTER(C.c_int64)),
+        ("read_ps", C.POINTER(C.c_int64)),
+        ("read_off", _u64p),
+        ("entry_pos", C.POINTER(C.c_int64)),
+        ("entry_allele", C.POINTER(C.c_int64)),
+        ("entry_quality", C.POINTER(C.c_int32)),
+        ("n_runs_pos", C.c_uint64),
+        ("runs_sample", C.POINTER(C.c_uint32)),
+        ("runs_pos", C.POINTER(C.c_int64)),
+        ("run_off", _u64p),
+        ("run_ps", C.POINTER(C.c_int64)),
+        ("run_h", C.POINTER(C.c_int64)),
+        ("run_score", C.POINTER(C.c_int64)),
+        ("gap_threshold", C.c_double),
+        ("only_indels", C.c_int32),
+    ]
+
+
+class CHaplotagphaseOutput(C.Structure):
+    """whmec_haplotagphase_output: caller-allocated per-sample arrays, library-allocated per-position arrays (released by
+    whmec_haplotagphase_release)."""
+    _fields_ = [
+        ("voted_off", _u64p),
+        ("skipped", _u64p),
+        ("entry_error", C.POINTER(C.c_int32)),
+        ("entry_error_at", _u64p),
+        ("n_voted", C.c_uint64),
+        ("voted_pos", C.POINTER(C.c_int64)),
+        ("phase_set", C.POINTER(C.c_int64)),
+        ("haplotype", C.POINTER(C.c_int64)),
+        ("score", C.POINTER(C.c_int64)),
+        ("total", C.POINTER(C.c_int64)),
+        ("allele", C.POINTER(C.c_int64)),
+        ("kept", _u8p),
+        ("error", C.POINTER(C.c_int32)),
+        ("key_off", _u64p),
+        ("key_ps", C.POINTER(C.c_int64)),
+        ("key_score", C.POINTER(C.c_int64)),
+    ]
+
+
+class CHaplotagphaseStats(C.Structure):
+    _fields_ = [
+        ("entries", C.c_uint64),
+        ("positions", C.c_uint64),
+        ("records", C.c_uint64),
+        ("h2d_bytes", C.c_uint64),
+        ("d2h_bytes", C.c_uint64),
+        ("chunks", C.c_uint32),
+        ("kernel_launches", C.c_uint32),
+        ("device_ms", C.c_float),
+        ("plan_ms", C.c_float),
+    ]
+
+    def as_dict(self) -> dict:
+        return {name: getattr(self, name) for name, _ in self._fields_}

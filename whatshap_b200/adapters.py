@@ -410,3 +410,23 @@ def make_prepare_haplotag_information(haplotag_module):
                                  linked_read_cutoff, ploidy, device, stats, library)
 
     return prepare_haplotag_information
+
+
+def make_haplotagphase(haplotagphase_module):
+    """(`compute_votes`, `consensus`) of whatshap_b200.haplotagphase that build `haplotagphase_module`'s own `Variant` and warn
+    through its `logger`, so that assigning them in place of the reference's functions leaves `run_haplotagphase` unchanged:
+
+        import whatshap.cli.haplotagphase as h, whatshap_b200.adapters as a
+        h.compute_votes, h.consensus = a.make_haplotagphase(h)
+    """
+    from . import haplotagphase
+
+    def compute_votes(is_homozygous, reads, allele_to_id, *, device=0, stats=None, library=None):
+        return haplotagphase._compute_votes(is_homozygous, reads, allele_to_id, haplotagphase_module.logger, device, stats, library)
+
+    def consensus(only_indels, gap_threshold, cut_homopolymers, refseq, change, phased, votes, id_to_allele, *, device=0, stats=None,
+                  library=None):
+        return haplotagphase._consensus(haplotagphase_module.Variant, only_indels, gap_threshold, cut_homopolymers, refseq, change, phased,
+                                        votes, id_to_allele, device, stats, library)
+
+    return compute_votes, consensus
