@@ -26,6 +26,7 @@
  *   whmec_learn            <- Caller (the k-mer pair counts of `whatshap learn`)  src/caller.cpp, whatshap/core.pyx:651-671
  *   whmec_haplotag         <- prepare_haplotag_information (read assignment of `whatshap haplotag`)  whatshap/cli/haplotag.py:322-427
  *   whmec_haplotagphase    <- compute_votes + best_candidate + consensus (`whatshap haplotagphase`)  whatshap/cli/haplotagphase.py:203-395
+ *   whmec_merge_reads      <- ReadMerger.merge (`whatshap phase --merge-reads`)  whatshap/merge.py:40-207
  *
  * Plain pointers and sizes only.  All input pointers are caller-owned host
  * memory, read-only, and need to stay valid only for the duration of the call.
@@ -651,6 +652,61 @@ typedef struct whmec_haplotagphase_stats {
 int whmec_haplotagphase(const whmec_haplotagphase_input *in, int device, whmec_haplotagphase_output *out, whmec_haplotagphase_stats *stats,
                         char *err, size_t errlen);
 void whmec_haplotagphase_release(whmec_haplotagphase_output *out);
+
+/* ---- Read merging of `whatshap phase --merge-reads`: ReadMerger.merge (whatshap/merge.py) for many readsets in one call.  Per
+ * set, read i has begin = its first position and end = begin + its number of entries; read j < i is compared with i iff
+ * end_j > begin_k for every k in (j, i].  The pair counts match m and mismatch mm over alleles_j[begin_i - begin_j:] (Python slice
+ * semantics) against alleles_i; the edge is blue when m + mm >= thr_neg_diff, min(m, mm) / (m + mm) <= max_error_rate and
+ * m - mm >= thr_diff, and also not-blue when in addition mm - m >= thr_neg_diff.  For every not-blue edge inside one blue
+ * component the blue edge of least m - mm on a bidirectional BFS path is removed until its ends part.  A blue component of two
+ * reads or more becomes one read at its least member: per position the qualities of each allele summed (z0, z1), allele
+ * z0 < z1, quality |z1 - z0|, positions ascending.  The host finds the pairs and cuts them into chunks under the free HBM less
+ * 512 MB (or WHMEC_MERGE_ARENA_BUDGET bytes); the device packs alleles as bits, evaluates one pair per thread, hooks blue
+ * edges into a parent array when no not-blue edge can exist (thr_diff + thr_neg_diff > 0; else the edges come back to the host
+ * for the removal loop), and sums the merged reads' entries by (representative, position) with a radix sort. */
+typedef struct whmec_merge_input {
+    uint32_t n_sets;
+    const uint64_t *set_off;         /* [n_sets + 1] into the reads */
+    const uint64_t *read_off;        /* [set_off[n_sets] + 1] into the entries */
+    const int32_t *position;
+    const uint8_t *allele;
+    const int32_t *quality;
+    int64_t thr_diff;
+    int64_t thr_neg_diff;
+    double max_error_rate;
+} whmec_merge_input;
+
+typedef struct whmec_merge_output {
+    int32_t *error_kind;             /* caller-allocated [n_sets]: 0 none, 1 IndexError (an empty read), 2 AssertionError (an allele
+                                        other than 0 or 1); a set with an error has no output reads */
+    uint64_t *error_read;            /* caller-allocated [n_sets]: the first offending read, an index within its set */
+    int64_t *representative;         /* caller-allocated [set_off[n_sets]]: every read's least component member, within its set */
+    uint64_t *out_off;               /* caller-allocated [n_sets + 1] into the output reads */
+    /* library-allocated, freed by whmec_merge_reads_release */
+    uint64_t n_out;
+    uint64_t *out_read;              /* [n_out]: the input read (a singleton or a representative), an index within its set */
+    uint64_t *out_entry_off;         /* [n_out + 1] into the output entries */
+    int32_t *out_position;
+    uint8_t *out_allele;
+    int64_t *out_quality;
+} whmec_merge_output;
+
+typedef struct whmec_merge_stats {
+    uint64_t reads, entries, pairs;
+    uint64_t blue_edges, notblue_edges, removed_edges;
+    uint64_t merged_components;      /* blue components of two reads or more */
+    uint64_t output_reads;
+    uint64_t h2d_bytes, d2h_bytes;
+    uint32_t chunks, kernel_launches;
+    float device_ms;                 /* device time of the launches (CUDA events) */
+    float plan_ms;                   /* host validation, pair counts, chunk cut, removal loop and output layout */
+} whmec_merge_stats;
+
+/* Returns WHMEC_OK (also when error_kind is set), WHMEC_ERR_INPUT for malformed arguments, WHMEC_ERR_UNSUPPORTED when a set has
+ * 2^32 reads or more, WHMEC_ERR_CUDA for a device failure.  stats may be NULL. */
+int whmec_merge_reads(const whmec_merge_input *in, int device, whmec_merge_output *out, whmec_merge_stats *stats, char *err,
+                      size_t errlen);
+void whmec_merge_reads_release(whmec_merge_output *out);
 
 #ifdef __cplusplus
 }

@@ -15,8 +15,9 @@ from .core import (  # noqa: F401
     get_max_genotype_alleles,
     get_max_genotype_ploidy,
 )
-from . import haplotag, haplotagphase  # noqa: F401
+from . import haplotag, haplotagphase, merge  # noqa: F401
 from .learn import Caller, count_kmer_pairs, write_counts  # noqa: F401
+from .merge import DoNothingReadMerger, ReadMerger, ReadMergerBase, merge_reads  # noqa: F401
 from .types import PhasingAlgorithm  # noqa: F401
 from .variant import Variant  # noqa: F401
 
@@ -26,5 +27,5 @@ PhasingAlgorithm.register(PedMecHeuristic)
 __all__ = [
     "Genotype", "GenotypeDPTable", "NumericSampleIds", "Pedigree", "PedigreeDPTable", "PedMecHeuristic", "PhredGenotypeLikelihoods", "Read", "ReadSet",
     "Variant", "PhasingAlgorithm", "compute_genotypes", "Caller", "count_kmer_pairs", "write_counts", "haplotag",
-    "haplotagphase",
+    "haplotagphase", "merge", "merge_reads", "ReadMerger", "ReadMergerBase", "DoNothingReadMerger",
 ]

@@ -567,3 +567,57 @@ class CHaplotagphaseStats(C.Structure):
 
     def as_dict(self) -> dict:
         return {name: getattr(self, name) for name, _ in self._fields_}
+
+
+class CMergeInput(C.Structure):
+    """whmec_merge_input: the reads of several readsets as CSR, and the edge rule's thresholds."""
+    _fields_ = [
+        ("n_sets", C.c_uint32),
+        ("set_off", _u64p),
+        ("read_off", _u64p),
+        ("position", C.POINTER(C.c_int32)),
+        ("allele", _u8p),
+        ("quality", C.POINTER(C.c_int32)),
+        ("thr_diff", C.c_int64),
+        ("thr_neg_diff", C.c_int64),
+        ("max_error_rate", C.c_double),
+    ]
+
+
+class CMergeOutput(C.Structure):
+    """whmec_merge_output: caller-allocated per-set and per-read arrays, library-allocated output reads (released by
+    whmec_merge_reads_release)."""
+    _fields_ = [
+        ("error_kind", C.POINTER(C.c_int32)),
+        ("error_read", _u64p),
+        ("representative", C.POINTER(C.c_int64)),
+        ("out_off", _u64p),
+        ("n_out", C.c_uint64),
+        ("out_read", _u64p),
+        ("out_entry_off", _u64p),
+        ("out_position", C.POINTER(C.c_int32)),
+        ("out_allele", _u8p),
+        ("out_quality", C.POINTER(C.c_int64)),
+    ]
+
+
+class CMergeStats(C.Structure):
+    _fields_ = [
+        ("reads", C.c_uint64),
+        ("entries", C.c_uint64),
+        ("pairs", C.c_uint64),
+        ("blue_edges", C.c_uint64),
+        ("notblue_edges", C.c_uint64),
+        ("removed_edges", C.c_uint64),
+        ("merged_components", C.c_uint64),
+        ("output_reads", C.c_uint64),
+        ("h2d_bytes", C.c_uint64),
+        ("d2h_bytes", C.c_uint64),
+        ("chunks", C.c_uint32),
+        ("kernel_launches", C.c_uint32),
+        ("device_ms", C.c_float),
+        ("plan_ms", C.c_float),
+    ]
+
+    def as_dict(self) -> dict:
+        return {name: getattr(self, name) for name, _ in self._fields_}

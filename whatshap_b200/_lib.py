@@ -13,7 +13,7 @@ from typing import List, Optional, Sequence, Tuple, Union
 
 import numpy as np
 
-from ._abi import CHaplotagInput, CHaplotagOutput, CHaplotagphaseInput, CHaplotagphaseOutput, CHaplotagphaseStats, CHaplotagStats, CHeuristicSolution, CKmeraldParams, CLearnInput, CLearnOutput, CLearnStats, CProblem, CQueryQualities, CRealignInput, CRealignOutput, CRealignStats, CSolution, CStats, FlatProblem, FlatSolution, HeuristicSolution, raise_for
+from ._abi import CHaplotagInput, CHaplotagOutput, CHaplotagphaseInput, CHaplotagphaseOutput, CHaplotagphaseStats, CHaplotagStats, CHeuristicSolution, CKmeraldParams, CLearnInput, CLearnOutput, CLearnStats, CMergeInput, CMergeOutput, CMergeStats, CProblem, CQueryQualities, CRealignInput, CRealignOutput, CRealignStats, CSolution, CStats, FlatProblem, FlatSolution, HeuristicSolution, raise_for
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("WHMEC_LIBRARY") or os.path.join(HERE, "libwhmec.so")  # WHMEC_LIBRARY: another build of the same library (A/B runs)
@@ -63,6 +63,8 @@ EXPORTS = (
     "whmec_haplotag",
     "whmec_haplotagphase",
     "whmec_haplotagphase_release",
+    "whmec_merge_reads",
+    "whmec_merge_reads_release",
 )
 
 
@@ -141,6 +143,7 @@ def lib() -> C.CDLL:
     learn_signatures(L)
     haplotag_signatures(L)
     haplotagphase_signatures(L)
+    merge_reads_signatures(L)
     for name in ("whmec_genotype_segment_create", "whmec_genotype_segment_transfer", "whmec_genotype_segment_run"):
         getattr(L, name).restype = C.c_int
     for name in ("whmec_plan_create", "whmec_plan_sweep", "whmec_plan_finish", "whmec_plan_stats", "whmec_solve",
@@ -208,6 +211,15 @@ def haplotagphase_signatures(L: C.CDLL) -> C.CDLL:
     L.whmec_haplotagphase.restype = C.c_int
     L.whmec_haplotagphase_release.argtypes = [C.POINTER(CHaplotagphaseOutput)]
     L.whmec_haplotagphase_release.restype = None
+    return L
+
+
+def merge_reads_signatures(L: C.CDLL) -> C.CDLL:
+    """argtypes of whmec_merge_reads and whmec_merge_reads_release on `L` (this library or a test build)."""
+    L.whmec_merge_reads.argtypes = [C.POINTER(CMergeInput), C.c_int, C.POINTER(CMergeOutput), C.POINTER(CMergeStats), C.c_char_p, C.c_size_t]
+    L.whmec_merge_reads.restype = C.c_int
+    L.whmec_merge_reads_release.argtypes = [C.POINTER(CMergeOutput)]
+    L.whmec_merge_reads_release.restype = None
     return L
 
 

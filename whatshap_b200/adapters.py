@@ -430,3 +430,27 @@ def make_haplotagphase(haplotagphase_module):
                                         votes, id_to_allele, device, stats, library)
 
     return compute_votes, consensus
+
+
+def make_read_merger(merge_module):
+    """A ReadMerger class of whatshap_b200.merge, constructed with the reference's positional arguments, that builds
+    `merge_module`'s own `Read` / `ReadSet` and logs through its `logger`, so that assigning it in place of the reference's
+    class leaves `whatshap phase --merge-reads` unchanged:
+
+        import whatshap.cli.phase, whatshap.merge, whatshap_b200.adapters as a
+        whatshap.cli.phase.ReadMerger = a.make_read_merger(whatshap.merge)
+    """
+    from . import merge
+
+    base = getattr(merge_module, "ReadMergerBase", object)
+    build = lambda m: merge._foreign_readset(m, merge_module.Read, merge_module.ReadSet)
+
+    class ReadMerger(base):
+        def __init__(self, error_rate, max_error_rate, positive_threshold, negative_threshold, *, device=0, stats=None, library=None):
+            self._params = (error_rate, max_error_rate, positive_threshold, negative_threshold)
+            self._device, self._stats, self._library = device, stats, library
+
+        def merge(self, readset):
+            return merge._merge(self._params, readset, build, merge_module.logger, self._device, self._stats, self._library)
+
+    return ReadMerger
